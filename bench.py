@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the SpeechT5 hot path on B200: BASELINE.json metric "utterances/sec (TTS fine-tune step, 10s@16kHz)".
+"""Benchmark of the SpeechT5 hot path on H100: BASELINE.json metric "utterances/sec (TTS fine-tune step, 10s@16kHz)".
 
   python bench.py --gpus N --steps K --warmup W            # our arm (one process per GPU under torchrun for N>1)
   python bench.py --impl reference --gpus N --steps K ...  # the reference math (CPU oracle port) on the host cores
@@ -16,6 +16,7 @@ import os
 import statistics
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -48,6 +49,9 @@ def parse():
     ap.add_argument("--exchange", default=None, choices=["shard", "allreduce"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-batch", type=int, default=2)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="tts workload: after the timed steps, write what the last timed update computed (loss, "
+                         "logging statistics, a fixed seeded sample of the updated fp32 parameters) as DIR/<name>.npy")
     ap.add_argument("--profile-step", action="store_true",
                     help="run 2 eager warm-up updates, then ONE eager update between cudaProfilerStart/Stop and exit "
                          "(for `ncu --profile-from-start off`); prints no bench line")
@@ -122,8 +126,9 @@ def run_reference(args, emit=True):
         opt.step()
         return loss.item()
 
-    warm = 1
-    steps = max(1, min(args.steps, 10)) if emit else 8  # ~10-15 s of CPU work: a bounded sample of the same workload
+    # as its own arm (--impl reference) it runs exactly --warmup + --steps updates; as the cpu_baseline field of our arm
+    # it times a fixed sample of 1 + 8 updates (~20 s of CPU work), whatever the GPU leg's step count
+    warm, steps = (args.warmup, args.steps) if emit else (1, 8)
     for _ in range(warm):
         step()
     t0 = time.time()
@@ -206,11 +211,29 @@ def _timed_steps(trainer, batches, steps, warmup, world, dev, read_back):
     return ms, (w0, w1), last, out
 
 
+# NVIDIA's H100 SXM data sheet (dense, a card allowed 700 W): a bound, not a rate reached -- a card with a lower power
+# limit runs below it under sustained load
+H100_PEAKS = {"bf16_tflops": 989.0, "hbm_gbs": 3350.0}
+H100_PEAK_SOURCE = "H100 SXM data sheet, dense BF16 (700 W card)"
+
+
 def _peaks():
-    try:
-        return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:  # noqa: BLE001
-        return {}
+    return H100_PEAKS
+
+
+def _dump_outputs(dirname, out, trainer):
+    """What the last timed update computed: the loss and logging statistics train_step returns, and a fixed seeded
+    sample of 2^20 elements of the updated fp32 master parameters (the whole flat vector is ~0.6 GB)."""
+    import numpy as np
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    flat = trainer.fp.flat
+    g = torch.Generator().manual_seed(20240601)
+    idx = torch.randint(0, flat.numel(), (1 << 20,), generator=g).sort().values
+    arrays = {"loss": out[0], "stats": out[1], "params_sample": flat[idx.to(flat.device)]}
+    for name, t in arrays.items():
+        if t is not None:
+            np.save(os.path.join(dirname, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 def _fresh_runtime(dtype, seed):
@@ -275,13 +298,13 @@ def parity_leg(args, dev, world):
     B = args.batch
     resident = [_to_device(synthetic_tts_batch(B, WORKLOAD["text_len"], WORKLOAD["mel_frames"], seed=i), dev)
                 for i in range(2)]
-    steps = max(3, min(args.steps, 6))
-    ms, _, _, out = _timed_steps(trainer, resident, steps, 3, 1, dev, read_back=False)
+    steps = args.steps
+    ms, _, _, out = _timed_steps(trainer, resident, steps, args.warmup, 1, dev, read_back=False)
     loss = float(out[0][0].item())
     del trainer, model
     torch.cuda.empty_cache()
     return {"value": B / (ms * 1e-3), "unit": "utterances/s", "ms_per_step": ms, "steps": steps, "loss": loss,
-            "dtype": "f32 activations, 3-pass split-bf16 tcgen05 GEMMs, fp32 row-kernel attention"}
+            "dtype": "f32 activations, 3-pass split-bf16 wgmma GEMMs, fp32 row-kernel attention"}
 
 # ------------------------------------------------------------------------------------------------ our arm
 def _finish(world):
@@ -307,7 +330,7 @@ def _emit(line, world):
 def run_asr(args):
     """BASELINE config 3: SpeechT5-Base ASR fine-tune step, 8 x 10 s waveforms per GPU -> 499 frames, 160 target tokens,
     CE + CTC (0.5 / 0.5, label smoothing 0.1), HuBERT time + channel masks, feature_grad_mult 1.0, LayerDrop 0.1 / 0.1,
-    dropout 0.1 -- the t5_transformer_base_asr recipe. Same JSON contract; `roofline` is the tcgen05 GEMM set of the
+    dropout 0.1 -- the t5_transformer_base_asr recipe. Same JSON contract; `roofline` is the wgmma GEMM set of the
     step, `roofline_conv0` the HBM-bound first conv layer (SURVEY 8d: 33.4 MB algorithmic per utterance, forward)."""
     import torch
     import torch.distributed as dist
@@ -394,8 +417,8 @@ def run_asr(args):
     conv0_ms = e0.elapsed_time(e1) / 20
     conv0_bytes = B * (2 * ASR["n_samples"] * 4 + y0.shape[1] * y0.shape[2] * 2)  # waveform read by both passes + bf16 store
     peaks = _peaks()
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_bw = peaks.get("hbm_gbs", 6500.0)
+    peak_tf = peaks["bf16_tflops"]
+    peak_bw = peaks["hbm_gbs"]
     clocks = sampler.window(*win_dev) if sampler else None
     if sampler:
         sampler.stop()
@@ -415,12 +438,12 @@ def run_asr(args):
                                "(device keep mask under the captured graph), clip 25, Adam",
                    "global_batch": utt, "parallelism": f"dp{world}", "exchange": trainer.exchange,
                    "cuda_graph": not args.no_graph, "loss": loss_val, "graphs_captured": trainer.graph_misses,
-                   "l2": "4 distinct input batches are cycled; the step's activations exceed the 126 MB L2"},
+                   "l2": "4 distinct input batches are cycled; the step's activations exceed the 50 MB L2"},
         "e2e": {"value": e2e, "unit": "utterances/s", "ms_per_step": ms_e2e, "h2d_bytes_per_step": h2d_bytes(host[0]),
                 "d2h_bytes_per_step": int(last.numel() * 4)},
         "gpu_launches": launches_step * args.steps, "gpu_launches_per_step": launches_step, "clocks": clocks,
         "step_tflops": ASR_GFLOP_PER_UTT_STEP * value / 1e3,
-        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_tcgen05 (all GEMM launches of one step)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_wgmma (all GEMM launches of one step)",
                      "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf,
                      "traffic": None, "launches": len(records), "gemm_ms_per_step": gemm_ms,
                      "gemm_share_of_step": gemm_ms / ms_dev},
@@ -538,7 +561,7 @@ def run_pretrain(args):
     e1.record()
     torch.cuda.synchronize()
     gemm_ms = e0.elapsed_time(e1) / 3
-    peak_tf = _peaks().get("bf16_tflops_sustained", 1400.0)
+    peak_tf = _peaks()["bf16_tflops"]
     clocks = sampler.window(*win_dev) if sampler else None
     if sampler:
         sampler.stop()
@@ -561,12 +584,12 @@ def run_pretrain(args):
                    "global_batch": per_update, "parallelism": f"dp{world}", "exchange": trainer.exchange,
                    "cuda_graph": False, "parameters": n_params, "losses_speech_text": losses,
                    "extractor_mode": margs.extractor_mode, "peak_memory_gib": torch.cuda.max_memory_allocated() / 2**30,
-                   "l2": "2 distinct input pairs are cycled; the update's activations exceed the 126 MB L2"},
+                   "l2": "2 distinct input pairs are cycled; the update's activations exceed the 50 MB L2"},
         "e2e": {"value": e2e, "unit": "samples/s", "ms_per_step": ms_e2e,
                 "h2d_bytes_per_step": sum(h2d_bytes(s) for s in host[0]), "d2h_bytes_per_step": int(last.numel() * 4)},
         "gpu_launches": launches_step * args.steps, "gpu_launches_per_step": launches_step, "clocks": clocks,
         "step_tflops": PRETRAIN_GFLOP_PER_UPDATE * world / 1e3 / (ms_dev * 1e-3),
-        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_tcgen05 (all GEMM launches of one update)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_wgmma (all GEMM launches of one update)",
                      "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf,
                      "traffic": None, "launches": len(records), "gemm_ms_per_step": gemm_ms,
                      "gemm_share_of_step": gemm_ms / ms_dev},
@@ -629,11 +652,11 @@ def run_hifigan(args):
                 out_host[: y.shape[0]].copy_(y.float(), non_blocking=True)
             n += y.numel()
         return n
-    for _ in range(max(1, args.warmup // 2)):
+    for _ in range(args.warmup):
         run(True)
     torch.cuda.synchronize()
     K.LAUNCHES = 0
-    reps = max(1, args.steps // 10)
+    reps = args.steps
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     sampler = ClockSampler(local) if rank == 0 else None
     w0 = time.time()
@@ -664,10 +687,10 @@ def run_hifigan(args):
         return
     samples = 512 * 204800
     peaks = _peaks()
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
+    peak_tf = peaks["bf16_tflops"]
     tf = 512 * 218.65e9 / (ms * 1e-3) / 1e12
     line = {"metric": "waveform samples/sec (HiFi-GAN vocoder inference)", "value": samples / (ms * 1e-3),
-            "unit": "samples/s", "n_gpus": world, "steps": reps, "warmup": max(1, args.warmup // 2), "ms_per_step": ms,
+            "unit": "samples/s", "n_gpus": world, "steps": reps, "warmup": args.warmup, "ms_per_step": ms,
             "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": "HiFi-GAN generator (BASELINE config 5): 512 x [800, 80] mels -> 512 x 204800 samples, "
                                    f"chunks of {chunk}; rates 4.4.4.4, 512 initial channels, resblock kernels 3/7/11",
@@ -675,7 +698,7 @@ def run_hifigan(args):
             "e2e": {"value": samples / (ms_e2e * 1e-3), "unit": "samples/s", "ms_per_step": ms_e2e,
                     "h2d_bytes_per_step": 512 * 800 * 80 * 4, "d2h_bytes_per_step": samples * 4},
             "gpu_launches": launches * reps, "gpu_launches_per_step": launches, "clocks": clocks,
-            "roofline": {"bound": "tensor", "kernel": "gemm_bf16_tcgen05 window GEMMs (every convolution of the generator)",
+            "roofline": {"bound": "tensor", "kernel": "gemm_bf16_wgmma window GEMMs (every convolution of the generator)",
                          "achieved": tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": tf / peak_tf, "traffic": None,
                          "note": "whole-generator figure: 218.65 GFLOP per utterance (SURVEY 8d) / wall time of the pass; "
                                  "layer-by-layer execution moves 0.94 GB of bf16 activations per utterance"}}
@@ -758,6 +781,8 @@ def run_ragged(args):
 
 def main():
     args = parse()
+    if args.dump_outputs and (args.workload != "tts" or args.impl != "b200"):
+        raise SystemExit("--dump-outputs: the tts workload of our arm only")
     if args.impl == "reference":
         run_reference(args)
         return
@@ -809,8 +834,9 @@ def main():
         trainer.train_step([resident[2]])
         torch.cuda.synchronize()
         torch.cuda.profiler.stop()
-        os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-        with open(os.path.join(ROOT, "gpurun_out", "gemm_shapes.json"), "w") as fh:  # launch-ordered, joins the ncu list
+        shapes = os.path.join(tempfile.mkdtemp(prefix="st5_profile_"), "gemm_shapes.json")
+        print("GEMM shapes of the profiled update:", shapes, file=sys.stderr)
+        with open(shapes, "w") as fh:  # launch-ordered, joins the profiler's kernel list
             json.dump([dict(M=g.M, N=g.N, K=g.K, nb=g.nb1 * g.nb2, a_mn=g.a_mn, b_mn=g.b_mn, c_fp32=g.c_fp32,
                             acc=g.accumulate, act=g.act, drop=g.drop_p > 0, pre=bool(g.c_pre), ag=bool(g.actgrad_pre))
                        for g in K.GEMM_RECORD], fh)
@@ -823,6 +849,8 @@ def main():
     ms_dev, win_dev, _, out = timed(resident, read_back=False)
     launches_step = None
     ms_e2e, win_e2e, last, out = timed(host, read_back=True)
+    if args.dump_outputs and rank == 0:
+        _dump_outputs(args.dump_outputs, out, trainer)
     loss_val = float(out[0][0].item())
     # kernels launched per step: counted once while the step was traced (graph mode replays the same launches)
     K.LAUNCHES = 0
@@ -836,7 +864,7 @@ def main():
         dist.barrier()
     launches_step = K.LAUNCHES
     records, K.GEMM_RECORD = K.GEMM_RECORD, None
-    # ---- roofline of the dominant kernel (the tcgen05 GEMM): replay exactly this step's GEMM launches back to back
+    # ---- roofline of the dominant kernel (the wgmma GEMM): replay exactly this step's GEMM launches back to back
     gemm_flops = sum(2.0 * g.M * g.N * g.K * g.nb1 * g.nb2 for g in records)
     K.gemm_replay(records)
     torch.cuda.synchronize()
@@ -853,24 +881,10 @@ def main():
     e1.record()
     torch.cuda.synchronize()
     gemm_ms = e0.elapsed_time(e1) / reps
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:  # noqa: BLE001
-        pass
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (measured)" if peaks else "fallback 1.4 PF sustained"
+    peak_tf = _peaks()["bf16_tflops"]
+    peak_src = H100_PEAK_SOURCE
     achieved_tf = gemm_flops / (gemm_ms * 1e-3) / 1e12
-    # DRAM traffic of the same kernel from the committed ncu pass (profiles/, per launch like `achieved`): measured
-    # under ncu (cold L2 per launch), so it is an upper bound of what the warm step moves
-    traffic, traffic_note = None, "no ncu traffic file committed"
-    try:
-        tpath = os.path.join(ROOT, "profiles", "r02_gemm_traffic.json")
-        tj = json.load(open(tpath if os.path.exists(tpath) else os.path.join(ROOT, "profiles", "r01_gemm_traffic.json")))
-        traffic = tj["dram_bytes_per_launch"]
-        traffic_note = tj.get("note", "")
-    except Exception:  # noqa: BLE001
-        pass
+    traffic, traffic_note = None, "not measured"
     clocks = sampler.window(*win_dev) if sampler else None
     if sampler:
         sampler.stop()
@@ -890,7 +904,7 @@ def main():
                    "global_batch": utt_per_step, "params": nparams, "parallelism": f"dp{world}",
                    "exchange": trainer.exchange, "cuda_graph": not args.no_graph, "loss": loss_val,
                    "l2": "per-step working set (>3 GB activations + 0.9 GB parameter/optimizer state) exceeds the "
-                         "126 MB L2; 4 distinct input batches are cycled"},
+                         "50 MB L2; 4 distinct input batches are cycled"},
         "e2e": {"value": e2e, "unit": "utterances/s", "ms_per_step": ms_e2e,
                 "h2d_bytes_per_step": h2d_bytes(host[0]), "d2h_bytes_per_step": int(last.numel() * 4),
                 "input_pipeline": "B200Trainer.prefetch: the next step's pinned batch is copied host->device on a copy "
@@ -900,7 +914,7 @@ def main():
         "clocks": clocks,
         # SURVEY 8(d): fwd/utt = text-encoder 29.07 + decoder 6.00/layer + pre/post-nets 2.36 GFLOP; step = 3x forward
         "step_tflops": 3.0 * (29.07 + 6.0 * args.decoder_layers + 2.36) * value / 1e3,
-        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_tcgen05 (all GEMM launches of one step)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_wgmma (all GEMM launches of one step)",
                      "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf,
                      "traffic": traffic, "traffic_note": traffic_note, "peak_source": peak_src,
                      "launches": len(records),

@@ -1,5 +1,5 @@
 /*
- * speecht5_b200 -- C ABI of the B200 (sm_100a) kernel library for the SpeechT5 forward/backward hot path.
+ * speecht5_b200 -- C ABI of the H100 (sm_90a) kernel library for the SpeechT5 forward/backward hot path.
  *
  * The reference (microsoft/SpeechT5, SpeechT5/speecht5/models/modules/*.py) has no FFI of its own: every device op is
  * a PyTorch library call made from the nn.Module forward()s. This header is the boundary a maintainer binds instead
@@ -39,12 +39,12 @@ extern "C" {
 
 int st5_version(void);
 const char* st5_last_error(void);
-/* sm_100a only: returns 0 when the current device can run the library, else a negative code. */
+/* sm_90a only: returns 0 when the current device can run the library, else a negative code. */
 int st5_device_ok(void);
 
 /* ------------------------------------------------------------------------------------------------- GEMM
- * D[z][m][n] = epi( alpha * sum_k A[z][m][k] * B[z][n][k] ), bf16 operands, fp32 accumulation in TMEM
- * (TMA + tcgen05.mma). Replaces every nn.Linear / torch.bmm / F.conv1d on the path:
+ * D[z][m][n] = epi( alpha * sum_k A[z][m][k] * B[z][n][k] ), bf16 operands, fp32 accumulation in registers
+ * (TMA + wgmma). Replaces every nn.Linear / torch.bmm / F.conv1d on the path:
  *   models/modules/multihead_attention.py:213-231 (q/k/v), :340 (QK^T), :389 (PV), :397 (out_proj);
  *   models/modules/transformer_layer.py:127-132, 385-391 (fc1/fc2);
  *   models/modules/speech_decoder_prenet.py:41-47,69-72; speech_decoder_postnet.py:31-32,39-51 (Conv1d as an
@@ -169,10 +169,10 @@ typedef struct st5_attn_args {
 int st5_attn_fwd(const st5_attn_args* args, void* stream);
 int st5_attn_bwd(const st5_attn_args* args, void* stream);
 
-/* Fused tcgen05 attention forward (bf16, Tk <= 320): QK^T -> masks -> softmax -> dropout -> PV in ONE launch, scores
- * resident in TMEM. Uses the q/k/v/out/probs/key_pad/scale/dropout fields of st5_attn_args exactly like st5_attn_fwd;
- * additionally writes lse[b][h][i] = log sum_j exp(scale*q_i.k_j) (may be NULL). probs (optional, only when the caller
- * wants them: need_head_weights) receives the undropped normalised probabilities in probs_dtype.
+/* Fused wgmma attention forward (bf16, Tk <= 320): QK^T -> masks -> softmax -> dropout -> PV in ONE launch, no score
+ * or probability round trip through HBM. Uses the q/k/v/out/probs/key_pad/scale/dropout fields of st5_attn_args exactly
+ * like st5_attn_fwd; additionally writes lse[b][h][i] = log sum_j exp(scale*q_i.k_j) (may be NULL). probs (optional,
+ * only when the caller wants them: need_head_weights) receives the undropped normalised probabilities in probs_dtype.
  * What the backward pass reads back (both optional, but together): psave [B,H,Tq,p_ld] BF16 = exp(s - rowmax), NOT
  * normalised, with the SIGN BIT set on elements dropout removed (probabilities are non-negative; a dropped zero is -0),
  * and inv_l [B,H,Tq] = 1 / rowsum. p_ld must be a multiple of 8, psave 16-byte aligned. out_f32 (optional)
@@ -181,17 +181,17 @@ int st5_attn_bwd(const st5_attn_args* args, void* stream);
  * Relative positions (encoder.py:239-246): pe_k != NULL selects the skewed-bias variant; here pe_k must point to a
  * BF16 copy of the [2*maxpos][64] table, and Tq, Tk <= maxpos <= 160 (clamp(i-j) never clips), no causal mask. */
 int st5_attn_fused_fwd(const st5_attn_args* args, float* lse, void* psave, float* inv_l, float* out_f32, void* stream);
-/* Streaming ("flash") tcgen05 attention forward for ANY Tq / Tk (bf16): 128-key blocks, the row maximum is made final
+/* Streaming ("flash") wgmma attention forward for ANY Tq / Tk (bf16): 64-key blocks, the row maximum is made final
  * in a first sweep over the key blocks (scores only), a second sweep computes exp / dropout / P V with the output
- * accumulating in TMEM, a third one (only when args->probs != NULL, which must then be FP32) writes the normalised
+ * accumulating in registers, a third one (only when args->probs != NULL, which must then be FP32) writes the normalised
  * probabilities. Same arguments, outputs and psave / inv_l / out_f32 contract as st5_attn_fused_fwd, so
  * st5_attn_fused_bwd is its backward. Relative positions: pe_k = BF16 copy of the [2*maxpos][64] table, any Tq / Tk --
  * clamp(i - j, -maxpos, maxpos - 1) clips as encoder.py:40-59 does; no causal mask together with pe_k. */
 int st5_attn_flash_fwd(const st5_attn_args* args, float* lse, void* psave, float* inv_l, float* out_f32, void* stream);
-/* Fused tcgen05 attention backward (multihead_attention.py:340-389 differentiated). psave / inv_l are what
+/* Fused wgmma attention backward (multihead_attention.py:340-389 differentiated). psave / inv_l are what
  * st5_attn_fused_fwd wrote: probabilities and dropout decisions are read back instead of recomputed (no exponential, no
- * Philox), so every step needs one score-sized MMA (dP = dO V^T) and the kernel double buffers dP, the dropout(P)/dS
- * operand tiles, dQ and the Q/dO tiles. Reads q/k/v, out (forward result), dout and drop_p; optional dprobs_ext (then
+ * Philox), so every step needs one score-sized MMA (dP = dO V^T); the Q / dO tiles and the saved exponentials are
+ * double buffered. Reads q/k/v, out (forward result), dout and drop_p; optional dprobs_ext (then
  * args->probs must be the FP32 probabilities the forward returned); writes dq/dk/dv (same layouts as q/k/v).
  * ext_heads > 0: dprobs_ext is known to be zero for heads >= ext_heads (the guided-attention loss reads the first two
  * heads of every layer, text_to_speech_loss.py:210-212) -- those heads skip its loads. out_f32 (optional): what the

@@ -117,7 +117,7 @@ def load():
         raise RuntimeError(
             f"speecht5_b200: CUDA library not found at {LIB_PATH}. Run `python -m speecht5_b200.build` "
             "(or __graft_entry__.build()). There is no CPU fallback for the product path.")
-    # ST5_LIB: an alternative build of the same ABI (tools/build_variant.sh makes A/B builds for tuning runs)
+    # ST5_LIB: an alternative build of the same ABI (A/B builds for tuning runs)
     lib = C.CDLL(os.environ.get("ST5_LIB") or LIB_PATH)
     for name, (res, args) in _PROTOS.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly

@@ -5,7 +5,7 @@ samples every hop, periodic-hann window, |rFFT|, Slaney mel projection, log10(ma
 The operand views are checked on the CPU through the GEMM emulator against oracle/audio_oracle.py
 (tests/test_frontend_cpu.py), the device path in tests/test_frontend_gpu.py.
 
-Device formulation: the STFT of every utterance is ONE batched tcgen05 GEMM -- row t of utterance b is the n_fft
+Device formulation: the STFT of every utterance is ONE batched wgmma GEMM -- row t of utterance b is the n_fft
 contiguous samples starting at t*hop of the padded waveform (row pitch = hop: overlapping windows, no framing copy),
 times a constant [2*(n_fft/2+1), n_fft] matrix holding the windowed cosine and negative sine bases -- in split precision
 (hi*hi + hi*lo + lo*hi of bf16 pairs, fp32 accumulate: measured 1e-3 worst case in the log10 domain,

@@ -1,6 +1,6 @@
-"""In-tree build of libspeecht5_b200.so (hand-written sm_100a kernels behind a C ABI, no torch dependency).
+"""In-tree build of libspeecht5_b200.so (hand-written sm_90a kernels behind a C ABI, no torch dependency).
 
-nvcc cross-compiles without a GPU; the resulting .so travels with the source tree (git-ignored, not gpurun-ignored).
+nvcc cross-compiles without a GPU; the resulting .so is written into the source tree (git-ignored).
 """
 import hashlib
 import os
@@ -10,11 +10,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libspeecht5_b200.so")
-SOURCES = ["api.cu", "gemm.cu", "elementwise.cu", "norm.cu", "layernorm.cu", "attention.cu", "attention_tc.cu", "attention_fused.cu", "attention_fused_bwd.cu", "attention_flash.cu",
+SOURCES = ["api.cu", "gemm.cu", "elementwise.cu", "norm.cu", "layernorm.cu", "attention.cu", "attention_tc.cu", "attention_fused_bwd.cu", "attention_flash.cu",
            "optim.cu", "conv_frontend.cu", "ctc.cu", "criterion.cu"]
 HEADERS = ["ptx.cuh", "gemm.cuh", "kernels.cuh", "tma_map.cuh", "vec8.cuh", os.path.join("..", "..", "include", "speecht5_b200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-cudart", "static",
 ]
 

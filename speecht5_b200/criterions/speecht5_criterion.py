@@ -80,7 +80,7 @@ class SpeechT5Criterion(FairseqCriterion):
             return self.text_pretrain_criterion(model, sample, reduce)
         if task_name == "speech_pretrain":
             return self.speech_pretrain_criterion(model, sample, reduce)
-        raise NotImplementedError(f"criterion branch '{task_name}' is not built in the B200 path (speaker identification)")
+        raise NotImplementedError(f"criterion branch '{task_name}' is not built in the H100 path (speaker identification)")
 
     # ------------------------------------------------------------------ logging (speecht5_criterion.py:123-436)
     @staticmethod

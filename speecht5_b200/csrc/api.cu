@@ -44,7 +44,7 @@ int st5_device_ok(void) {
   cudaDeviceProp prop;
   if (cudaGetDevice(&dev) != cudaSuccess) return set_error(-1, "st5_device_ok");
   if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return set_error(-1, "st5_device_ok");
-  if (prop.major != 10) return set_error(-2, "st5_device_ok: library is built for sm_100a only");
+  if (prop.major != 9) return set_error(-2, "st5_device_ok: library is built for sm_90a only");
   return 0;
 }
 

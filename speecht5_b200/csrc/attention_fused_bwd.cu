@@ -1,18 +1,15 @@
-// Fused attention backward on tcgen05. The probabilities come from the forward pass -- bf16 exp(s - rowmax) with the
-// dropout decision in the sign bit, normalised here by the saved 1/rowsum -- so one step needs a single score-sized MMA,
-// no exponential and no random numbers, and the schedule can be fully overlapped.
+// Fused attention backward on the Hopper tensor cores (wgmma). The probabilities come from the forward pass -- bf16
+// exp(s - rowmax) with the dropout decision in the sign bit, normalised here by the saved 1/rowsum -- so one step needs
+// a single score-sized MMA, no exponential and no random numbers.
 //
-// One CTA per (head, utterance). Loop: key block kb (128 keys) outer, query tile qt (128 rows) inner; step it:
-//   MMA1(it)   dP = dO_qt V_kb^T                     -> TMEM dP[it & 1]               (issued one step AHEAD)
-//   threads    (16 warps, 1 thread = 1 query row x 32 keys): dS = P * (dP_masked + dP_ext - delta);
-//              dropout(P) and dS -> shared memory tiles [it & 1] (bf16, 128B-swizzled [q][key])
-//   MMA2(it)   dV_kb += dropout(P)^T dO_qt, dK_kb += dS^T Q_qt   (A = the smem tiles read MN-major)
-//              dQ_qt(kb) = dS K_kb                    -> TMEM dQ[it & 1]
-//   threads    read-out of step it-1 (after the element phase of step it): dQ partial -> fp32 accumulator in HBM
-//              (plain RMW: the CTA owns its (b,h)), bf16 on the last key block; dK_kb / dV_kb after the last tile.
-// dP, the two smem tiles, dQ and the Q/dO buffers are all double buffered: while the threads work on step it, the tensor
-// core runs MMA2(it-1) and MMA1(it+1) and TMA fetches Q/dO(it+1). Every mbarrier belongs to one buffer and is waited
-// phase by phase in order (a parity wait on a barrier two phases behind would fall through).
+// One CTA per (head, utterance). Loop: key block kb (64 keys) outer, query tile qt (64 rows) inner; step it:
+//   MMA warpgroup  dP = dO_qt V_kb^T -> shared memory (fp32 rows)
+//   threads        (4 warps, 1 thread = 1 query row x 32 keys): dS = P * (dP_masked + dP_ext - delta);
+//                  dropout(P) and dS -> shared memory tiles (bf16, 128B-swizzled [q][key])
+//   MMA warpgroup  dV_kb += dropout(P)^T dO_qt, dK_kb += dS^T Q_qt (registers, the tiles read MN-major),
+//                  dQ_qt(kb) = dS K_kb -> fp32 accumulator in HBM straight from the fragments (plain RMW: the CTA owns
+//                  its (b,h)), bf16 on the last key block; dK_kb / dV_kb after the last query tile of the block.
+// Q / dO and the saved exponentials are double buffered: TMA fetches those of step it+1 while step it runs.
 // Semantics: backward of speecht5/models/modules/multihead_attention.py:340-389. With relative positions the two table
 // contractions dQ += dQP PE and dPE = dQP^T Q run on the batched GEMM from the dS written here.
 #include "../../include/speecht5_b200.h"
@@ -24,11 +21,11 @@ namespace st5 {
 
 int set_error(int code, const char* where);
 
-constexpr int FB_NG = 4;                       // compute warp groups: group g owns 32-key chunk g of the 128-key block
-constexpr int FB_THREADS = 64 + FB_NG * 128;  // TMA warp, MMA warp, 16 compute warps (4 per TMEM lane quarter)
-constexpr int FB_T = 128;  // query tile == key block
-constexpr size_t FB_SMEM = 6 * 16384 + 4 * 32768 + 256 + 1024;  // K V | Q x2 | dO x2 | dropout(P) x2 | dS x2 | barriers
-constexpr uint32_t FB_COL_DP = 0, FB_COL_DK = 256, FB_COL_DV = 320, FB_COL_DQ = 384;  // dP: 2 x 128, dQ: 2 x 64 columns
+constexpr int FB_T = 64;                 // query tile == key block
+constexpr int FB_THREADS = 9 * 32;       // MMA warpgroup, TMA warp, 4 compute warps
+constexpr int FB_DPP = FB_T + 4;         // floats per row of the dP tile (row-per-lane float4 reads: conflict-free)
+// K V | Q x2 | dO x2 | dropout(P) x2 | dS | dP | barriers
+constexpr size_t FB_SMEM = 2 * 8192 + 4 * 8192 + 2 * 8192 + 8192 + (size_t)FB_T * FB_DPP * 4 + 256 + 1024;
 
 struct FusedBwdParams {
   int B, H, Tq, Tk, causal;
@@ -129,55 +126,46 @@ __global__ void attn_delta_ext_kernel(const float* __restrict__ probs, const flo
   if (lane == 0) delta[row] += acc;
 }
 
-__global__ void __launch_bounds__(FB_THREADS, 1)  // (18 warps are allocated as 20: 96 registers is the ceiling)
+__global__ void __launch_bounds__(FB_THREADS, 1)
     attn_fused_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                           const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do,
                           const __grid_constant__ CUtensorMap map_p, const FusedBwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sK = smem;             // [128 keys][128 B]
-  uint8_t* sV = sK + 16384;
-  uint8_t* sQ = sV + 16384;       // 2 x [128 rows][128 B]
-  uint8_t* sdO = sQ + 32768;      // 2 x [128 rows][128 B]
-  uint8_t* sPd = sdO + 32768;     // 2 x (2 blocks of [128 rows][64 keys])
-  uint8_t* sdS = sPd + 65536;     // 2 x (2 blocks of [128 rows][64 keys])
-  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sdS + 65536);  // K/V of a key block landed
+  uint8_t* sK = smem;             // [64 keys][128 B]
+  uint8_t* sV = sK + 8192;
+  uint8_t* sQ = sV + 8192;        // 2 x [64 rows][128 B]
+  uint8_t* sdO = sQ + 16384;      // 2 x [64 rows][128 B]
+  uint8_t* sPd = sdO + 16384;     // 2 x [64 rows][64 keys]: the saved exponentials, overwritten in place by dropout(P)
+  uint8_t* sdS = sPd + 16384;     // [64 rows][64 keys]
+  float* sDP = reinterpret_cast<float*>(sdS + 8192);  // [64][FB_DPP]
+  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sDP + FB_T * FB_DPP);  // K/V of a key block landed
   uint64_t* bar_kvfree = bar_kv + 1;  // every MMA that reads this key block's K/V tiles has completed
   uint64_t* bar_qdo = bar_kv + 2;     // [2] Q/dO buffer filled
-  uint64_t* bar_qfree = bar_kv + 4;   // [2] Q/dO buffer consumed by MMA2
-  uint64_t* bar_dp = bar_kv + 6;      // [2] MMA1 complete: dP buffer valid
-  uint64_t* bar_pds = bar_kv + 8;     // [2] threads: dropout(P)/dS tiles written, dP buffer read
-  uint64_t* bar_mma2 = bar_kv + 10;   // [2] MMA2 complete: dQ buffer (and dK/dV) valid, smem tiles free
-  uint64_t* bar_tdone = bar_kv + 12;  // [2] threads: dQ buffer (and dK/dV) read out
-  uint64_t* bar_pin = bar_kv + 14;    // [2] the saved exponentials of a step have landed in sPd[buf] (TMA)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_kv + 16);
+  uint64_t* bar_qfree = bar_kv + 4;   // [2] Q/dO/exponential buffers consumed by the step's MMAs
+  uint64_t* bar_pin = bar_kv + 6;     // [2] the saved exponentials of a step have landed in sPd[buf] (TMA)
+  uint64_t* bar_dp = bar_kv + 8;      // dP of the step is in sDP
+  uint64_t* bar_pds = bar_kv + 9;     // threads: dropout(P)/dS tiles written, dP read
 
   const int warp = threadIdx.x >> 5;
   const int h = blockIdx.x, b = blockIdx.y;
   const int nkb = (p.Tk + FB_T - 1) / FB_T, nqt = (p.Tq + FB_T - 1) / FB_T;
 
-  if (warp == 0 && elect_one()) {
+  if (warp == 4 && elect_one()) {
     tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); tma_prefetch_desc(&map_do);
     tma_prefetch_desc(&map_p);
     mbar_init(bar_kv, 1); mbar_init(bar_kvfree, 1);
     for (int s = 0; s < 2; ++s) {
-      mbar_init(&bar_qdo[s], 1); mbar_init(&bar_qfree[s], 1); mbar_init(&bar_dp[s], 1);
-      mbar_init(&bar_pds[s], FB_NG * 4); mbar_init(&bar_mma2[s], 1); mbar_init(&bar_tdone[s], FB_NG * 4);
-      mbar_init(&bar_pin[s], 1);
+      mbar_init(&bar_qdo[s], 1); mbar_init(&bar_qfree[s], 1); mbar_init(&bar_pin[s], 1);
     }
+    mbar_init(bar_dp, 128);
+    mbar_init(bar_pds, 4);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   pdl_sync();  // (prologue done: nothing above touched global memory)
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ===================== TMA producer =====================
     if (elect_one()) {
       int it = 0, kbc = 0;
@@ -186,178 +174,124 @@ __global__ void __launch_bounds__(FB_THREADS, 1)  // (18 warps are allocated as 
         for (int qt = qt0; qt < nqt; ++qt, ++it) {
           const int buf = it & 1;
           if (qt == qt0) {
-            if (kbc > 0) mbar_wait(bar_kvfree, (uint32_t)((kbc - 1) & 1));  // MMAs of the previous key block are done
+            if (kbc > 0) mbar_wait_quiet(bar_kvfree, (uint32_t)((kbc - 1) & 1));  // MMAs of the previous key block are done
             ++kbc;
-            mbar_expect_tx(bar_kv, 32768);
+            mbar_expect_tx(bar_kv, 16384);
             tma_load_4d(sK, &map_k, bar_kv, 0, kb * FB_T, h, b);
             tma_load_4d(sV, &map_v, bar_kv, 0, kb * FB_T, h, b);
           }
-          if (it >= 2) mbar_wait(&bar_qfree[buf], (uint32_t)(((it >> 1) - 1) & 1));  // MMA2(it-2) has read this buffer
-          mbar_expect_tx(&bar_qdo[buf], 32768);
-          tma_load_4d(sQ + buf * 16384, &map_q, &bar_qdo[buf], 0, qt * FB_T, h, b);
-          tma_load_4d(sdO + buf * 16384, &map_do, &bar_qdo[buf], 0, qt * FB_T, h, b);
+          if (it >= 2) mbar_wait_quiet(&bar_qfree[buf], (uint32_t)(((it >> 1) - 1) & 1));  // step it-2 has read this buffer
+          mbar_expect_tx(&bar_qdo[buf], 16384);
+          tma_load_4d(sQ + buf * 8192, &map_q, &bar_qdo[buf], 0, qt * FB_T, h, b);
+          tma_load_4d(sdO + buf * 8192, &map_do, &bar_qdo[buf], 0, qt * FB_T, h, b);
           // the saved exponentials of this (query tile, key block) go straight into the operand tile the threads will
-          // overwrite in place with dropout(P): same [128 rows][64 keys] x 2, 128B-swizzled layout. MMA2(it-2) -- the
-          // last reader of sPd[buf] -- has completed (bar_qfree above). A 64-key block that starts beyond the row
-          // pitch is not loaded (nothing reads it: those chunks are dead and get zeros from the threads).
-          const int nblk = (kb * FB_T + 64 < (int)p.p_ld) ? 2 : 1;
-          mbar_expect_tx(&bar_pin[buf], (uint32_t)nblk * 16384u);
-          for (int blk = 0; blk < nblk; ++blk)
-            tma_load_4d(sPd + buf * 32768 + blk * 16384, &map_p, &bar_pin[buf], kb * FB_T + blk * 64, qt * FB_T, h, b);
+          // overwrite in place with dropout(P): [64 rows][64 keys], 128B-swizzled
+          mbar_expect_tx(&bar_pin[buf], 8192u);
+          tma_load_4d(sPd + buf * 8192, &map_p, &bar_pin[buf], kb * FB_T, qt * FB_T, h, b);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
+  } else if (warp < 4) {
+    // ===================== MMA warpgroup =====================
     const uint32_t aK = smem_u32(sK), aV = smem_u32(sV), aQ0 = smem_u32(sQ), adO0 = smem_u32(sdO);
-    const uint32_t aPd0 = smem_u32(sPd), adS0 = smem_u32(sdS);
-    // dP(j) = dO V^T into dP[j & 1]. That buffer was last read by the threads in step j-2, which this warp has
-    // already waited for (bar_pds) before issuing MMA2(j-2).
-    auto issue1 = [&](int j) {
-      const int buf = j & 1;
-      mbar_wait(&bar_qdo[buf], (uint32_t)((j >> 1) & 1));
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t adO = adO0 + (uint32_t)buf * 16384u;
-        const uint32_t id = umma_idesc_bf16(128, 128, 0, 0);
+    const uint32_t aPd0 = smem_u32(sPd), adS = smem_u32(sdS);
+    const int l = (int)lane_id(), w = warp;
+    const int r0 = 16 * w + (l >> 2);  // fragment rows r0, r0 + 8; columns 8 (i >> 2) + 2 (l & 3) + (i & 1)
+    float dk[32], dv[32];
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16(tmem + FB_COL_DP + (uint32_t)buf * 128u, umma_smem_desc(adO + k * 32, 16, 1024),
-                    umma_smem_desc(aV + k * 32, 16, 1024), id, k != 0);
-        umma_commit(&bar_dp[buf]);
-      }
-      __syncwarp();
-    };
+    for (int t = 0; t < 32; ++t) dk[t] = dv[t] = 0.f;
     int it = 0, kbc = 0;
     for (int kb = 0; kb < nkb; ++kb) {
       const int qt0 = p.causal ? kb : 0;
       if (qt0 >= nqt) continue;
-      mbar_wait(bar_kv, (uint32_t)(kbc & 1));
+      mbar_wait_quiet(bar_kv, (uint32_t)(kbc & 1));
       ++kbc;
-      issue1(it);
       for (int qt = qt0; qt < nqt; ++qt, ++it) {
         const int buf = it & 1;
-        if (qt + 1 < nqt) issue1(it + 1);  // one step ahead (same key block: K/V stay put)
-        mbar_wait(&bar_pds[buf], (uint32_t)((it >> 1) & 1));
-        if (it >= 2) mbar_wait(&bar_tdone[buf], (uint32_t)(((it >> 1) - 1) & 1));  // dQ[buf] of step it-2 read out
-        // first step of a key block overwrites dK/dV: the previous block's read-out (step it-1) must be over
-        if (qt == qt0 && it >= 1) mbar_wait(&bar_tdone[(it - 1) & 1], (uint32_t)(((it - 1) >> 1) & 1));
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t aQ = aQ0 + (uint32_t)buf * 16384u, adO = adO0 + (uint32_t)buf * 16384u;
-          const uint32_t aPd = aPd0 + (uint32_t)buf * 32768u, adS = adS0 + (uint32_t)buf * 32768u;
-          const uint32_t acc = qt != qt0;
-          const uint32_t id_t = umma_idesc_bf16(128, 64, 1, 1);  // A = P^T / dS^T (MN-major), B = dO / Q (MN-major)
+        const uint32_t aQ = aQ0 + (uint32_t)buf * 8192u, adO = adO0 + (uint32_t)buf * 8192u;
+        const uint32_t aPd = aPd0 + (uint32_t)buf * 8192u;
+        mbar_wait_quiet(&bar_qdo[buf], (uint32_t)((it >> 1) & 1));
+        {  // dP = dO V^T (A = dO, B = V: both K-major over the head dimension)
+          float dp[32];
+          wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 8; ++k) {  // contraction over the 128 query rows
-            umma_bf16(tmem + FB_COL_DV, umma_smem_desc(aPd + k * 2048, 16384, 1024),
-                      umma_smem_desc(adO + k * 2048, 16384, 1024), id_t, acc | (uint32_t)(k != 0));
-            umma_bf16(tmem + FB_COL_DK, umma_smem_desc(adS + k * 2048, 16384, 1024),
-                      umma_smem_desc(aQ + k * 2048, 16384, 1024), id_t, acc | (uint32_t)(k != 0));
-          }
-          const uint32_t id_q = umma_idesc_bf16(128, 64, 0, 1);  // A = dS (K-major), B = K (MN-major)
+          for (int k = 0; k < 4; ++k)
+            wgmma_m64n64<0, 0>(dp, wgmma_smem_desc(adO + k * 32, 16, 1024), wgmma_smem_desc(aV + k * 32, 16, 1024),
+                               k != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_regs(dp);
 #pragma unroll
-          for (int k = 0; k < 8; ++k) {  // contraction over the 128 keys: 2 blocks x 4 k-steps
-            const int blk = k >> 2, ks = k & 3;
-            umma_bf16(tmem + FB_COL_DQ + (uint32_t)buf * 64u, umma_smem_desc(adS + blk * 16384 + ks * 32, 16, 1024),
-                      umma_smem_desc(aK + (blk * 64 + ks * 16) * 128, 16384, 1024), id_q, k != 0);
+          for (int i = 0; i < 32; i += 2) {
+            const int rr = r0 + 8 * ((i >> 1) & 1), cc = 8 * (i >> 2) + 2 * (l & 3);
+            *reinterpret_cast<float2*>(sDP + rr * FB_DPP + cc) = make_float2(dp[i], dp[i + 1]);
           }
-          umma_commit(&bar_mma2[buf]);
-          umma_commit(&bar_qfree[buf]);
-          if (qt == nqt - 1) umma_commit(bar_kvfree);
         }
-        __syncwarp();
+        mbar_arrive(bar_dp);
+        mbar_wait_quiet(bar_pds, (uint32_t)(it & 1));
+        float dq[32];
+        wgmma_fence();
+        const uint32_t acc = qt != qt0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {  // contraction over the 64 query rows: A = P^T / dS^T, B = dO / Q (all MN-major)
+          wgmma_m64n64<1, 1>(dv, wgmma_smem_desc(aPd + k * 2048, 8192, 1024), wgmma_smem_desc(adO + k * 2048, 8192, 1024),
+                             acc | (uint32_t)(k != 0));
+          wgmma_m64n64<1, 1>(dk, wgmma_smem_desc(adS + k * 2048, 8192, 1024), wgmma_smem_desc(aQ + k * 2048, 8192, 1024),
+                             acc | (uint32_t)(k != 0));
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k)  // contraction over the 64 keys: A = dS (K-major), B = K (MN-major)
+          wgmma_m64n64<0, 1>(dq, wgmma_smem_desc(adS + k * 32, 16, 1024), wgmma_smem_desc(aK + k * 2048, 8192, 1024),
+                             k != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(dq);
+        wgmma_fence_regs(dk);
+        wgmma_fence_regs(dv);
+        if (threadIdx.x == 0) {
+          mbar_arrive(&bar_qfree[buf]);
+          if (qt == nqt - 1) mbar_arrive(bar_kvfree);
+        }
+        // ---- dQ partial of (kb, qt): running fp32 sum over the key blocks, bf16 after the last one
+        const int kb_last = p.causal ? (qt < nkb - 1 ? qt : nkb - 1) : nkb - 1;
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+          const int row = qt * FB_T + r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
+          if (row < p.Tq) {
+            float2 f = make_float2(dq[i] * p.scale, dq[i + 1] * p.scale);
+            float* accp = p.dq_acc + ((int64_t)b * p.Tq + row) * (p.H * 64) + h * 64 + col;
+            if (kb > 0) {
+              const float2 o = *reinterpret_cast<const float2*>(accp);
+              f.x += o.x; f.y += o.y;
+            }
+            if (kb == kb_last)
+              *reinterpret_cast<uint32_t*>(p.dq + (int64_t)b * p.q_bs + (int64_t)row * p.q_ld + h * 64 + col) = pack2(f.x, f.y);
+            else
+              *reinterpret_cast<float2*>(accp) = f;
+          }
+        }
+        if (qt == nqt - 1) {  // dK / dV of the key block
+#pragma unroll
+          for (int i = 0; i < 32; i += 2) {
+            const int key = kb * FB_T + r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
+            if (key < p.Tk) {
+              *reinterpret_cast<uint32_t*>(p.dk + (int64_t)b * p.k_bs + (int64_t)key * p.k_ld + h * 64 + col) =
+                  pack2(dk[i] * p.scale, dk[i + 1] * p.scale);
+              *reinterpret_cast<uint32_t*>(p.dv + (int64_t)b * p.v_bs + (int64_t)key * p.v_ld + h * 64 + col) =
+                  pack2(dv[i], dv[i + 1]);
+            }
+          }
+        }
       }
     }
   } else {
-    // ===================== compute threads (thread = query row / key row) =====================
-    const int q = warp & 3;
-    const int grp = (warp - 2) >> 2;  // 32-key chunk of the block, 16-channel slice of dQ, 32-channel slice of dK|dV
+    // ===================== compute threads (thread = query row x 32-key chunk) =====================
+    const int sw = warp - 5;
+    const int q = sw & 1;
+    const int c = sw >> 1;  // this warp's 32-key chunk of the block
     const int r = q * 32 + (int)lane_id();
-    const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16);
-    // this thread's 16 running dQ sums of query tile qt (written by this same thread one key block earlier)
-    float4 qpf[4];
-    auto prefetch_acc = [&](int kb, int qt) {
-      const int i = qt * FB_T + r;
-      if (kb > 0 && i < p.Tq) {
-        const float* acc = p.dq_acc + ((int64_t)b * p.Tq + i) * (p.H * 64) + h * 64 + grp * 16;
-#pragma unroll
-        for (int t = 0; t < 4; ++t) qpf[t] = *reinterpret_cast<const float4*>(acc + 4 * t);
-      }
-    };
-    // ---- read-out of one finished step: dQ partial of (kb, qt); dK / dV after the last query tile of a key block
-    auto read_out = [&](int kb, int qt, int j) {
-      const int buf = j & 1;
-      const int k0 = kb * FB_T;
-      const int i = qt * FB_T + r;
-      const bool row_ok = i < p.Tq;
-      mbar_wait(&bar_mma2[buf], (uint32_t)((j >> 1) & 1));
-      tc_fence_after();
-      const int kb_last = p.causal ? (qt < nkb - 1 ? qt : nkb - 1) : nkb - 1;
-      {
-        uint32_t v[16];
-        tmem_ld_32x16(trow + FB_COL_DQ + (uint32_t)(buf * 64 + grp * 16), v);
-        tmem_ld_wait();
-        if (row_ok) {
-          float* acc = p.dq_acc + ((int64_t)b * p.Tq + i) * (p.H * 64) + h * 64 + grp * 16;
-          float f[16];
-#pragma unroll
-          for (int t = 0; t < 16; ++t) f[t] = __uint_as_float(v[t]) * p.scale;
-          if (kb > 0) {  // running sum over the earlier key blocks (requested a whole element phase ago: prefetch_acc)
-#pragma unroll
-            for (int t = 0; t < 16; t += 4) {
-              const float4 o = qpf[t >> 2];
-              f[t] += o.x; f[t + 1] += o.y; f[t + 2] += o.z; f[t + 3] += o.w;
-            }
-          }
-          if (kb == kb_last) {
-            __nv_bfloat16* dst = p.dq + (int64_t)b * p.q_bs + (int64_t)i * p.q_ld + h * 64 + grp * 16;
-#pragma unroll
-            for (int t = 0; t < 16; t += 8) {
-              uint4 pk;
-              pk.x = pack2(f[t], f[t + 1]); pk.y = pack2(f[t + 2], f[t + 3]);
-              pk.z = pack2(f[t + 4], f[t + 5]); pk.w = pack2(f[t + 6], f[t + 7]);
-              *reinterpret_cast<uint4*>(dst + t) = pk;
-            }
-          } else {
-#pragma unroll
-            for (int t = 0; t < 16; t += 4)
-              *reinterpret_cast<float4*>(acc + t) = make_float4(f[t], f[t + 1], f[t + 2], f[t + 3]);
-          }
-        }
-      }
-      if (qt == nqt - 1) {  // thread = key row; groups 0,1 write the two 32-channel halves of dK, groups 2,3 those of dV
-        const int j_key = k0 + r;
-        uint32_t v[32];
-        tmem_ld_32x32(trow + (grp < 2 ? FB_COL_DK : FB_COL_DV) + (uint32_t)((grp & 1) * 32), v);
-        tmem_ld_wait();
-        if (j_key < p.Tk) {
-          const float sc = grp < 2 ? p.scale : 1.f;
-          __nv_bfloat16* dst = (grp < 2 ? p.dk + (int64_t)b * p.k_bs + (int64_t)j_key * p.k_ld
-                                        : p.dv + (int64_t)b * p.v_bs + (int64_t)j_key * p.v_ld) + h * 64 + (grp & 1) * 32;
-#pragma unroll
-          for (int t = 0; t < 32; t += 8) {
-            uint4 pk;
-            pk.x = pack2(__uint_as_float(v[t]) * sc, __uint_as_float(v[t + 1]) * sc);
-            pk.y = pack2(__uint_as_float(v[t + 2]) * sc, __uint_as_float(v[t + 3]) * sc);
-            pk.z = pack2(__uint_as_float(v[t + 4]) * sc, __uint_as_float(v[t + 5]) * sc);
-            pk.w = pack2(__uint_as_float(v[t + 6]) * sc, __uint_as_float(v[t + 7]) * sc);
-            *reinterpret_cast<uint4*>(dst + t) = pk;
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane_id() == 0) mbar_arrive(&bar_tdone[buf]);
-    };
-    // per-row constants of the NEXT step are requested one step ahead (two dependent global round trips per step less)
-    float delta_n = 0.f, invl_n = 0.f;
-    if (nkb > 0 && nqt > 0 && r < p.Tq) {
-      const int64_t pr0 = ((int64_t)b * p.H + h) * p.Tq + r;
-      delta_n = p.delta[pr0];
-      invl_n = p.inv_l[pr0];
-    }
-    int it = 0, pend_kb = -1, pend_qt = 0;
+    const int cbase = c * 4;
+    int it = 0;
     for (int kb = 0; kb < nkb; ++kb) {
       const int qt0 = p.causal ? kb : 0;
       const int k0 = kb * FB_T;
@@ -366,50 +300,41 @@ __global__ void __launch_bounds__(FB_THREADS, 1)  // (18 warps are allocated as 
         const int i = qt * FB_T + r;
         const bool row_ok = i < p.Tq;
         const int64_t prow = ((int64_t)b * p.H + h) * p.Tq + i;
-        const float delta = delta_n, invl = invl_n;
-        {
-          int kb2 = kb, qt2 = qt + 1;
-          if (qt2 >= nqt) { kb2 = kb + 1; qt2 = p.causal ? kb2 : 0; }
-          const int i2 = qt2 * FB_T + r;
-          delta_n = invl_n = 0.f;
-          if (kb2 < nkb && qt2 < nqt && i2 < p.Tq) {
-            const int64_t pr2 = ((int64_t)b * p.H + h) * p.Tq + i2;
-            delta_n = p.delta[pr2];
-            invl_n = p.inv_l[pr2];
-          }
-        }
-        if (pend_kb >= 0) prefetch_acc(pend_kb, pend_qt);  // for the read-out that follows this step's element phase
+        const float delta = row_ok ? p.delta[prow] : 0.f, invl = row_ok ? p.inv_l[prow] : 0.f;
         const float* dpx = (p.dp_ext != nullptr && row_ok && h < p.ext_heads) ? p.dp_ext + prow * p.p_ld : nullptr;
-        const int c = grp;  // this warp's 32-key chunk of the block
         const int col0 = k0 + c * 32;
-        mbar_wait(&bar_dp[buf], (uint32_t)((it >> 1) & 1));
-        tc_fence_after();
-        mbar_wait(&bar_pin[buf], (uint32_t)((it >> 1) & 1));  // the exponentials are in sPd[buf] (every warp: nobody
-                                                               // may write the tile before the TMA has)
-        uint8_t* bp = sPd + buf * 32768 + (c >> 1) * 16384 + r * 128;
-        uint8_t* bs = sdS + buf * 32768 + (c >> 1) * 16384 + r * 128;
-        const int cbase = (c & 1) * 4;
+        mbar_wait_quiet(bar_dp, (uint32_t)(it & 1));
+        mbar_wait_quiet(&bar_pin[buf], (uint32_t)((it >> 1) & 1));  // the exponentials are in sPd[buf] (every warp:
+                                                                    // nobody may write the tile before the TMA has)
+        uint8_t* bp = sPd + buf * 8192 + r * 128;
+        uint8_t* bs = sdS + r * 128;
         // warp-uniform fast path: no live query row in this warp's 32 rows, or the whole key chunk lies beyond Tk --
         // P is zero there, so both operand tiles get zeros (they are contracted over, so they must be written)
         const bool dead = (qt * FB_T + q * 32 >= p.Tq) || (col0 >= p.Tk);
         if (dead) {
 #pragma unroll
           for (int g = 0; g < 4; ++g) {
-            const int sw = ((cbase + g) ^ (r & 7)) << 4;
-            *reinterpret_cast<uint4*>(bp + sw) = make_uint4(0u, 0u, 0u, 0u);
-            *reinterpret_cast<uint4*>(bs + sw) = make_uint4(0u, 0u, 0u, 0u);
+            const int swz = ((cbase + g) ^ (r & 7)) << 4;
+            *reinterpret_cast<uint4*>(bp + swz) = make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>(bs + swz) = make_uint4(0u, 0u, 0u, 0u);
             if (p.ds_out != nullptr && row_ok && col0 + 8 * g + 8 <= p.p_ld)
               *reinterpret_cast<uint4*>(p.ds_out + prow * p.p_ld + col0 + 8 * g) = make_uint4(0u, 0u, 0u, 0u);
           }
         } else {
         // (dP is finite everywhere: V rows beyond Tk and dO rows beyond Tq arrive as zeros from TMA)
-        uint32_t dv[32];
-        tmem_ld_32x32(trow + FB_COL_DP + (uint32_t)(buf * 128 + c * 32), dv);
-        tmem_ld_wait();
+        float dvv[32];
+        {
+          const float* src = sDP + r * FB_DPP + c * 32;
+#pragma unroll
+          for (int t = 0; t < 32; t += 4) {
+            const float4 f = *reinterpret_cast<const float4*>(src + t);
+            dvv[t] = f.x; dvv[t + 1] = f.y; dvv[t + 2] = f.z; dvv[t + 3] = f.w;
+          }
+        }
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
-          const int sw = ((cbase + g) ^ (r & 7)) << 4;
-          const uint4 praw = *reinterpret_cast<const uint4*>(bp + sw);  // this row's 8 saved exponentials (in place)
+          const int swz = ((cbase + g) ^ (r & 7)) << 4;
+          const uint4 praw = *reinterpret_cast<const uint4*>(bp + swz);  // this row's 8 saved exponentials (in place)
           const uint32_t w4[4] = {praw.x, praw.y, praw.z, praw.w};
           float xd[8];
           xd[0] = xd[1] = xd[2] = xd[3] = xd[4] = xd[5] = xd[6] = xd[7] = 0.f;
@@ -437,7 +362,7 @@ __global__ void __launch_bounds__(FB_THREADS, 1)  // (18 warps are allocated as 
               const float keepf = (int32_t)raw < 0 ? 0.f : p.drop_scale;      // sign bit = dropped by the forward pass
               const float pv = fabsf(__uint_as_float(raw)) * invl;           // the probability
               // dP as the softmax sees it: dropout backward of dO V^T, plus the caller's gradient
-              const float dp = __uint_as_float(dv[8 * g + t]) * keepf + xd[t];
+              const float dp = dvv[8 * g + t] * keepf + xd[t];
               pd8[t] = pv * keepf;
               ds8[t] = pv * (dp - delta);
             }
@@ -445,39 +370,24 @@ __global__ void __launch_bounds__(FB_THREADS, 1)  // (18 warps are allocated as 
           uint4 a, d;
           a.x = pack2(pd8[0], pd8[1]); a.y = pack2(pd8[2], pd8[3]); a.z = pack2(pd8[4], pd8[5]); a.w = pack2(pd8[6], pd8[7]);
           d.x = pack2(ds8[0], ds8[1]); d.y = pack2(ds8[2], ds8[3]); d.z = pack2(ds8[4], ds8[5]); d.w = pack2(ds8[6], ds8[7]);
-          *reinterpret_cast<uint4*>(bp + sw) = a;
-          *reinterpret_cast<uint4*>(bs + sw) = d;
+          *reinterpret_cast<uint4*>(bp + swz) = a;
+          *reinterpret_cast<uint4*>(bs + swz) = d;
           if (p.ds_out != nullptr && row_ok && col0 + 8 * g + 8 <= p.p_ld)
             *reinterpret_cast<uint4*>(p.ds_out + prow * p.p_ld + col0 + 8 * g) = d;
         }
         }
         fence_proxy_async();
-        tc_fence_before();
         __syncwarp();
-        if (lane_id() == 0) mbar_arrive(&bar_pds[buf]);
-        // ---- the previous step's accumulators are read while the tensor core works on this step and the next
-        if (pend_kb >= 0) read_out(pend_kb, pend_qt, it - 1);
-        pend_kb = kb;
-        pend_qt = qt;
+        if (lane_id() == 0) mbar_arrive(bar_pds);
       }
     }
-    if (pend_kb >= 0) {
-      prefetch_acc(pend_kb, pend_qt);
-      read_out(pend_kb, pend_qt, it - 1);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
   }
 }
 
-static int make_map128(CUtensorMap* m, const void* ptr, int64_t rows, int64_t ld, int64_t bs, int H, int B) {
+static int make_map64(CUtensorMap* m, const void* ptr, int64_t rows, int64_t ld, int64_t bs, int H, int B) {
   const uint64_t dims[4] = {64, (uint64_t)rows, (uint64_t)H, (uint64_t)B};
   const uint64_t strides[3] = {(uint64_t)ld * 2, 128, (uint64_t)bs * 2};
-  const uint32_t box[4] = {64, 128, 1, 1};
+  const uint32_t box[4] = {64, FB_T, 1, 1};
   return encode_bf16_map_4d(m, ptr, dims, strides, box);
 }
 
@@ -506,7 +416,7 @@ extern "C" int st5_attn_fused_bwd(const st5_attn_args* a, const void* psave, con
     return set_error(-4, "st5_attn_fused_bwd: out / dout must be 16-byte aligned");
   const int eh = ext_heads > 0 && ext_heads < a->H ? ext_heads : a->H;
   // external dP on a few heads only (and vector-loadable outputs): every row takes the cheap dO.O path, a second small
-  // launch adds sum_j P dP_ext on the rows of those heads (33.7 -> ~15 us per guided layer at the benched shape)
+  // launch adds sum_j P dP_ext on the rows of those heads only
   const bool split = ext && eh < a->H && !((a->o_ld & 7) || (a->o_bs & 7) || (reinterpret_cast<uintptr_t>(a->dout) & 15) ||
                                            (reinterpret_cast<uintptr_t>(a->out) & 15));
   const int64_t warps_needed = (ext && !split) ? nrows : (nrows + 3) / 4;
@@ -522,14 +432,14 @@ extern "C" int st5_attn_fused_bwd(const st5_attn_args* a, const void* psave, con
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error((int)e, "st5_attn_fused_bwd(delta)");
   CUtensorMap mq, mk, mv, mdo, mp;
-  int rc = make_map128(&mq, a->q, a->Tq, a->q_ld, a->q_bs, a->H, a->B);
-  if (!rc) rc = make_map128(&mk, a->k, a->Tk, a->k_ld, a->k_bs, a->H, a->B);
-  if (!rc) rc = make_map128(&mv, a->v, a->Tk, a->v_ld, a->v_bs, a->H, a->B);
-  if (!rc) rc = make_map128(&mdo, a->dout, a->Tq, a->o_ld, a->o_bs, a->H, a->B);
-  if (!rc) {  // psave [B][H][Tq][p_ld] bf16: boxes of 64 keys x 128 query rows, out-of-range rows / columns read as zero
+  int rc = make_map64(&mq, a->q, a->Tq, a->q_ld, a->q_bs, a->H, a->B);
+  if (!rc) rc = make_map64(&mk, a->k, a->Tk, a->k_ld, a->k_bs, a->H, a->B);
+  if (!rc) rc = make_map64(&mv, a->v, a->Tk, a->v_ld, a->v_bs, a->H, a->B);
+  if (!rc) rc = make_map64(&mdo, a->dout, a->Tq, a->o_ld, a->o_bs, a->H, a->B);
+  if (!rc) {  // psave [B][H][Tq][p_ld] bf16: boxes of 64 keys x 64 query rows, out-of-range rows / columns read as zero
     const uint64_t dims[4] = {(uint64_t)a->p_ld, (uint64_t)a->Tq, (uint64_t)a->H, (uint64_t)a->B};
     const uint64_t strides[3] = {(uint64_t)a->p_ld * 2, (uint64_t)a->Tq * a->p_ld * 2, (uint64_t)a->H * a->Tq * a->p_ld * 2};
-    const uint32_t box[4] = {64, 128, 1, 1};
+    const uint32_t box[4] = {64, FB_T, 1, 1};
     rc = encode_bf16_map_4d(&mp, psave, dims, strides, box);
   }
   if (rc) return set_error(rc, "st5_attn_fused_bwd: tensor map");

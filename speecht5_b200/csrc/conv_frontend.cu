@@ -70,7 +70,7 @@ __global__ void conv0_stats_kernel(const float* __restrict__ wave, const float* 
 
 // Chan's pairwise combination of the per-chunk (sum, M2) in double: mean / rstd per (utterance, channel).
 // block (64 channels, 8 chunk groups), grid (B, C / 64): the ~250 chunks of a 10 s utterance are walked by 8 threads per
-// channel and met in shared memory (the one-thread-per-channel form ran 8 CTAs for 156 us).
+// channel and met in shared memory (one thread per channel would leave the grid at 8 CTAs).
 constexpr int C0_FG = 8;
 __global__ void __launch_bounds__(64 * C0_FG)
     conv0_finalize_kernel(const float* __restrict__ part, float* __restrict__ mean, float* __restrict__ rstd, int T0,
@@ -495,7 +495,7 @@ int conv0_bwd_launch(const void* dy, const float* wave, const float* w, const fl
 
 // ---- layer_norm mode launchers
 static inline int c0l_grid(int64_t frames, int per_cta) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t want = (frames + per_cta - 1) / per_cta;

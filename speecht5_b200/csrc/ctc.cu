@@ -5,8 +5,7 @@
 //   1 ctc_rows_kernel   (warp per (t, b) row)  lse_t = logsumexp_k logits[t,b,k];  lp[b,t,s] = logits[t,b,l'_s] - lse_t
 //   2 ctc_sweeps_kernel (CTA per utterance)    alpha (forward) and beta (backward) recursions run CONCURRENTLY in the two
 //                       halves of the CTA, one thread per state, one barrier per time step; the emission terms lp are
-//                       fetched a group of steps ahead (the per-step global round trip was the whole cost of the
-//                       one-sweep-after-the-other form: 1.8 us per step);
+//                       fetched a group of steps ahead (a global round trip per step would dominate the recursion);
 //                         alpha_t(s) = lp_t(s) + lse(alpha_{t-1}(s), alpha_{t-1}(s-1), [alpha_{t-1}(s-2) if l'_s != blank, != l'_{s-2}])
 //                         beta_t(s)  = lp_t(s) + lse(beta_{t+1}(s),  beta_{t+1}(s+1),  [beta_{t+1}(s+2)  if l'_s != blank, != l'_{s+2}])
 //                       nll = -lse of the two final alpha states

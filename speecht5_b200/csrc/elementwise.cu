@@ -9,7 +9,7 @@ namespace st5 {
 
 static inline int grid_for(int64_t n, int threads) {
   int64_t g = (n + threads - 1) / threads;
-  return (int)(g > 148 * 32 ? 148 * 32 : (g < 1 ? 1 : g));
+  return (int)(g > 132 * 32 ? 132 * 32 : (g < 1 ? 1 : g));
 }
 
 // ------------------------------------------------------------------ fp32 -> bf16 (hi [, lo])
@@ -407,7 +407,7 @@ int colsum_launch(const void* x, int64_t ld, float* out, int dtype, int64_t rows
   const int64_t cw = vec_ok ? 32 * vec : 32;  // columns per block
   const int64_t col_blocks = (cols + cw - 1) / cw;
   // enough row splits to fill the machine a few times over, each split at least 64 rows deep
-  int64_t splits = (4 * 148 + col_blocks * groups - 1) / (col_blocks * groups);
+  int64_t splits = (4 * 132 + col_blocks * groups - 1) / (col_blocks * groups);
   const int64_t max_splits = (group_rows + 63) / 64;
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;

@@ -1,8 +1,9 @@
-// Batched bf16 GEMM on the 5th-generation tensor cores (tcgen05.mma, accumulators in TMEM), operands staged by
-// TMA into 128B-swizzled shared memory through an mbarrier ring. One CTA computes a 128 x BN output tile.
+// Batched bf16 GEMM on the Hopper tensor cores (wgmma, fp32 accumulators in registers), operands staged by TMA into
+// 128B-swizzled shared memory through an mbarrier ring. One CTA computes a 128 x BN output tile.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = MMA issuer (+ TMEM allocation), warps 2..5 =
-// epilogue (TMEM -> registers -> fused bias / activation / dropout / residual -> global).
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread), warpgroups 1..2 = consumers: each issues
+// the wgmma of 64 rows of the tile, then all 8 consumer warps run the epilogue (accumulators -> swizzled shared
+// memory -> one row x 32 columns per thread -> fused bias / activation / dropout / residual -> global).
 //
 // This one kernel is the contraction engine for every dense op on the SpeechT5 path: the q/k/v/out projections
 // (reference: speecht5/models/modules/multihead_attention.py:213-231,397), the FFN (transformer_layer.py:127-132,
@@ -22,9 +23,9 @@ namespace st5 {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 bytes = one swizzle row
-constexpr int UMMA_K = 16;
-constexpr int EPI_WARPS = 16;  // epilogue warps: 4 per TMEM lane quarter, each taking every 4th 32-column chunk
-constexpr int GEMM_THREADS = 64 + 32 * EPI_WARPS;
+constexpr int MMA_K = 16;
+constexpr int EPI_WARPS = 8;  // the consumer warps: 4 row quarters x 2 column groups, each taking every 2nd 32-column chunk
+constexpr int GEMM_THREADS = 128 + 32 * EPI_WARPS;
 
 struct EpiParams {
   int M, N, nb1;
@@ -71,110 +72,107 @@ __device__ __forceinline__ void actgrad8(float* v, const uint4 u) {
   }
 }
 
-// CTAS = 2 (SURVEY section 8f / DESIGN section 8 item 1): the two CTAs of a cluster -- the two SMs of one TPC -- share a
-// 256 x BN output tile. Each stages its own 128 rows of A and BN/2 columns of B (a third less operand traffic per
-// output element than 128 x 256), the leader's MMA warp issues tcgen05.mma.cta_group::2 for both, and each CTA drains
-// its own 128 accumulator rows. All pipeline barriers that cross the pair live in the leader's shared memory.
-template <int BN, int STAGES, bool A_MN, bool B_MN, int CTAS>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap map_a,
-                                                                  const __grid_constant__ CUtensorMap map_b,
-                                                                  const __grid_constant__ CUtensorMap map_c,
-                                                                  const __grid_constant__ CUtensorMap map_cpre,
-                                                                  const EpiParams p) {
+template <int BN, bool A_MN, bool B_MN>
+__device__ __forceinline__ void gemm_mainloop(float (&acc)[BN / 2], const uint8_t* smem_a, const uint8_t* smem_b,
+                                              uint64_t* full_bar, uint64_t* empty_bar, int& stage, uint32_t& phase,
+                                              int nkb, int wg, int STAGES) {
   constexpr uint32_t A_BYTES = BLOCK_M * BLOCK_K * 2;
-  constexpr int B_ROWS = BN / CTAS;  // B columns (= rows of the [N, K] operand) this CTA stages
-  constexpr uint32_t B_BYTES = B_ROWS * BLOCK_K * 2;
+  constexpr uint32_t B_BYTES = BN * BLOCK_K * 2;
+  constexpr uint32_t CHUNK_BYTES = 64 * BLOCK_K * 2;  // one 64(mn) x 64(k) MN-major box
+  const bool leader = (threadIdx.x & 127) == 0;
+  int prev = -1;
+  for (int kb = 0; kb < nkb; ++kb) {
+    mbar_wait_quiet(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(smem_a + stage * A_BYTES) + (uint32_t)wg * 8192u;  // this warpgroup's 64 rows
+    const uint32_t sb = smem_u32(smem_b + stage * B_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+      // K-major: advance 16 elements (32 B) along the swizzled row. MN-major: advance 16 k-rows (2 KB).
+      const uint64_t da = A_MN ? wgmma_smem_desc(sa + k * (MMA_K * 128), CHUNK_BYTES, 1024)
+                               : wgmma_smem_desc(sa + k * (MMA_K * 2), 16, 1024);
+      const uint64_t db = B_MN ? wgmma_smem_desc(sb + k * (MMA_K * 128), CHUNK_BYTES, 1024)
+                               : wgmma_smem_desc(sb + k * (MMA_K * 2), 16, 1024);
+      if constexpr (BN == 128) wgmma_m64n128<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+      else wgmma_m64n64<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    // keep one k-block of MMAs in flight: the slot of the previous one is free once it has retired
+    wgmma_wait<1>();
+    wgmma_fence_regs(acc);
+    if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+  if (leader) mbar_arrive(&empty_bar[prev]);
+}
+
+// fp32 accumulator tile in shared memory, [BLOCK_M][BN] with the 16-byte column groups of row r XOR-ed by r % 8:
+// the epilogue's row-per-lane float4 reads are conflict-free.
+template <int BN>
+__device__ __forceinline__ int acc_idx(int row, int col) {
+  return row * BN + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3));
+}
+
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(32 * EPI_WARPS) : "memory"); }
+
+template <int BN, int STAGES, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_wgmma(const __grid_constant__ CUtensorMap map_a,
+                                                                const __grid_constant__ CUtensorMap map_b,
+                                                                const __grid_constant__ CUtensorMap map_c,
+                                                                const __grid_constant__ CUtensorMap map_cpre,
+                                                                const EpiParams p) {
+  constexpr uint32_t A_BYTES = BLOCK_M * BLOCK_K * 2;
+  constexpr uint32_t B_BYTES = BN * BLOCK_K * 2;
   constexpr uint32_t CHUNK_BYTES = 64 * BLOCK_K * 2;  // one 64(mn) x 64(k) MN-major box
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_BYTES;
-  uint8_t* stg_all = smem_b + STAGES * B_BYTES;  // EPI_WARPS x 4 KB staging blocks for the TMA-store epilogue
+  float* sacc = reinterpret_cast<float*>(smem_b + STAGES * B_BYTES);        // BLOCK_M x BN fp32 accumulators
+  uint8_t* stg_all = reinterpret_cast<uint8_t*>(sacc + BLOCK_M * BN);        // EPI_WARPS x 4 KB TMA-store staging
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_all + EPI_WARPS * 4096);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;   // [2] accumulator stage complete (MMA -> epilogue)
-  uint64_t* tempty_bar = tfull_bar + 2;       // [2] accumulator stage drained (epilogue -> MMA)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   // Persistent CTA: loops over output tiles (m fastest, so concurrently running CTAs share the B/weight tile in L2);
-  // two TMEM accumulator stages let the epilogue of tile i overlap the MMA main loop of tile i+1.
+  // the producer runs ahead into the next tile while the consumers drain the current one.
   const int warp = threadIdx.x >> 5;
   const int nkb = p.num_k_blocks;
   const int tiles_mn = p.tiles_m * p.tiles_n;
-  const int rank = CTAS == 2 ? (int)cluster_ctarank() : 0;           // 0 = leader of the pair
-// first tile / stride of this CTA (pair) in the persistent schedule -- kept as expressions, not locals, so that the
-// single-CTA instantiations compile to the code they had before the pair variant existed
-#define ST5_TILE0 (CTAS == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x)
-#define ST5_TILE_STEP (CTAS == 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x)
-  constexpr int TILE_M = BLOCK_M * CTAS;
 
   if (warp == 0 && elect_one()) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], EPI_WARPS * CTAS);  // one arrive per epilogue warp (of both CTAs of a pair)
+      mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if constexpr (CTAS == 2) cluster_sync_all();  // both CTAs of the pair are resident before the paired TMEM allocation
-  if (warp == 1) {
-    if constexpr (CTAS == 2) {
-      tmem_alloc_pair(tmem_slot, 2 * BN);
-      tmem_relinquish_pair();
-    } else {
-      tmem_alloc(tmem_slot, 2 * BN);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CTAS == 2) cluster_sync_all();  // the peer's barriers exist before anything is signalled across
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch: everything above touched only this CTA's shared / tensor memory, so it may run
-  // while the preceding grid drains. Wait for that grid's memory here, before the first global access, and let the
-  // grid behind us start its own prologue (both are no-ops when the launch carries no programmatic attribute).
+  // Programmatic dependent launch: everything above touched only this CTA's shared memory, so it may run while the
+  // preceding grid drains. Wait for that grid's memory here, before the first global access, and let the grid behind
+  // us start its own prologue (both are no-ops when the launch carries no programmatic attribute).
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = ST5_TILE0; tile < p.num_tiles; tile += ST5_TILE_STEP) {
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const int z = tile / tiles_mn, rmn = tile - z * tiles_mn;
-      const int m0 = (rmn % p.tiles_m) * TILE_M + rank * BLOCK_M, n0 = (rmn / p.tiles_m) * BN + rank * B_ROWS;
+      const int m0 = (rmn % p.tiles_m) * BLOCK_M, n0 = (rmn / p.tiles_m) * BN;
       const int b1 = z % p.nb1, b2 = z / p.nb1;
       for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_wait_quiet(&empty_bar[stage], phase ^ 1);
         uint8_t* sa = smem_a + stage * A_BYTES;
         uint8_t* sb = smem_b + stage * B_BYTES;
         const int k0 = kb * BLOCK_K;
-        if constexpr (CTAS == 2) {
-          // both producers credit the LEADER's full barrier, which expects the bytes of both halves of the stage
-          const uint32_t fb = mapa_u32(smem_u32(&full_bar[stage]), 0);
-          if (rank == 0) mbar_expect_tx(&full_bar[stage], 2 * (A_BYTES + B_BYTES));
-          if (A_MN) {
-#pragma unroll
-            for (int c = 0; c < BLOCK_M / 64; ++c)
-              tma_load_4d_pair(sa + c * CHUNK_BYTES, &map_a, fb, m0 + c * 64, k0, b1 * p.a_m1, b2 * p.a_m2);
-          } else {
-            tma_load_4d_pair(sa, &map_a, fb, k0, m0, b1 * p.a_m1, b2 * p.a_m2);
-          }
-          if (B_MN) {
-#pragma unroll
-            for (int c = 0; c < B_ROWS / 64; ++c)
-              tma_load_4d_pair(sb + c * CHUNK_BYTES, &map_b, fb, n0 + c * 64, k0, b1 * p.b_m1, b2 * p.b_m2);
-          } else {
-            tma_load_4d_pair(sb, &map_b, fb, k0, n0, b1 * p.b_m1, b2 * p.b_m2);
-          }
-        } else {
         mbar_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
         if (A_MN) {
 #pragma unroll
@@ -190,113 +188,59 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_tcgen05(const __gri
         } else {
           tma_load_4d(sb, &map_b, &full_bar[stage], k0, n0, b1 * p.b_m1, b2 * p.b_m2);
         }
-        }
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
       }
-      if constexpr (CTAS == 2) {
-        // tail: the leader's multicast commits arrive on THIS CTA's empty barriers; stay until every slot has been
-        // released so that none of them lands in the shared memory of a CTA that already left
-#pragma unroll 1
-        for (int i = 0; i < STAGES; ++i) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = umma_idesc_bf16(TILE_M, BN, A_MN ? 1 : 0, B_MN ? 1 : 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int local = 0;
-    // (pair: only the leader's MMA warp issues; the peer's warp 1 just owns its half of the TMEM allocation)
-    for (int tile = (CTAS == 2 && rank != 0) ? p.num_tiles : ST5_TILE0; tile < p.num_tiles; tile += ST5_TILE_STEP, ++local) {
-    const int acc = local & 1;
-    const uint32_t acc_phase = (uint32_t)(local >> 1) & 1u;
-    const uint32_t tmem_acc = tmem_base + (uint32_t)(acc * BN);
-    mbar_wait(&tempty_bar[acc], acc_phase ^ 1);  // epilogue has drained this accumulator stage
-    tc_fence_after();
-    for (int kb = 0; kb < nkb; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa = smem_u32(smem_a + stage * A_BYTES);
-        const uint32_t sb = smem_u32(smem_b + stage * B_BYTES);
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-          // K-major: advance 16 elements (32 B) along the swizzled row. MN-major: advance 16 k-rows (2 KB).
-          const uint64_t da = A_MN ? umma_smem_desc(sa + k * (UMMA_K * 128), CHUNK_BYTES, 1024)
-                                   : umma_smem_desc(sa + k * (UMMA_K * 2), 16, 1024);
-          const uint64_t db = B_MN ? umma_smem_desc(sb + k * (UMMA_K * 128), CHUNK_BYTES, 1024)
-                                   : umma_smem_desc(sb + k * (UMMA_K * 2), 16, 1024);
-          if constexpr (CTAS == 2) umma_bf16_pair(tmem_acc, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-          else umma_bf16(tmem_acc, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        if constexpr (CTAS == 2) {  // the same barrier offsets in both CTAs of the pair
-          umma_commit_pair(&empty_bar[stage], 3);
-          if (kb == nkb - 1) umma_commit_pair(&tfull_bar[acc], 3);
-        } else {
-        umma_commit(&empty_bar[stage]);                     // smem slot reusable once these MMAs retire
-        if (kb == nkb - 1) umma_commit(&tfull_bar[acc]);    // accumulator complete
-        }
-      }
-      __syncwarp();
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-    }
     }
   } else {
-    // ===================== epilogue (4 warps, one TMEM lane quarter each) =====================
-    const int q = warp & 3;                      // TMEM lane quarter this warp may read (hardware: warp id % 4)
+    // ===================== consumers: wgmma main loop, then the epilogue =====================
+    setmaxnreg_inc<232>();
+    const int cw = warp - 4;                     // consumer warp 0..7
+    const int wg = cw >> 2;                      // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
+    const int q = cw & 3;                        // epilogue: row quarter [32 q, 32 q + 32)
     constexpr int NGRP = EPI_WARPS / 4;
-    const int grp = (warp - 2) >> 2;             // which 32-column chunks this warp owns: c = grp, grp + NGRP, ...
-    uint8_t* stg = stg_all + (warp - 2) * 4096;
+    const int grp = cw >> 2;                     // epilogue: 32-column chunks c = grp, grp + NGRP, ...
+    uint8_t* stg = stg_all + cw * 4096;
     uint64_t dseed = p.drop_seed, doffset = p.drop_offset;
     if (p.drop_thr != 0) resolve_seed(dseed, doffset);
-    int local = 0;
-    for (int tile = ST5_TILE0; tile < p.num_tiles; tile += ST5_TILE_STEP, ++local) {
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
     const int z = tile / tiles_mn, rmn = tile - z * tiles_mn;
-    const int m0 = (rmn % p.tiles_m) * TILE_M + rank * BLOCK_M, n0 = (rmn / p.tiles_m) * BN;
+    const int m0 = (rmn % p.tiles_m) * BLOCK_M, n0 = (rmn / p.tiles_m) * BN;
     const int b1 = z % p.nb1, b2 = z / p.nb1;
-    const int acc = local & 1;
-    const uint32_t acc_phase = (uint32_t)(local >> 1) & 1u;
-    const uint32_t tmem_acc = tmem_base + (uint32_t)(acc * BN);
+    {
+      float acc[BN / 2];
+      gemm_mainloop<BN, A_MN, B_MN>(acc, smem_a, smem_b, full_bar, empty_bar, stage, phase, nkb, wg, STAGES);
+      consumer_sync();  // the previous tile's epilogue has read the accumulator tile
+      const int l = (int)lane_id();
+      const int rbase = wg * 64 + (cw & 3) * 16 + (l >> 2);
+#pragma unroll
+      for (int i = 0; i < BN / 2; i += 2) {
+        const int rr = rbase + 8 * ((i >> 1) & 1), cc = 8 * (i >> 2) + 2 * (l & 3);
+        *reinterpret_cast<float2*>(sacc + acc_idx<BN>(rr, cc)) = make_float2(acc[i], acc[i + 1]);
+      }
+      consumer_sync();
+    }
     const int row = m0 + q * 32 + (int)lane_id();
     const bool row_ok = row < p.M;
     const long zoff = (long)b1 * p.c_bs1 + (long)b2 * p.c_bs2;
     const long roff = zoff + (long)row * p.c_ld;
-    // (Requesting the gate / residual / bias of a chunk ahead of the accumulator wait was tried -- A/B build, round 2:
-    // the 16-24 extra live registers cost more in spills than the hidden latency gave back, +0.3 ms per step.)
-    mbar_wait(&tfull_bar[acc], acc_phase);
-    tc_fence_after();
     const float* bias2_row = (p.bias2 != nullptr && row_ok) ? p.bias2 + (long)(row / p.bias2_rows) * p.N : nullptr;
     const uint64_t drop_row = ((uint64_t)z * (uint64_t)p.M + (uint64_t)row) * (uint64_t)p.N;
-    if (grp >= BN / 32) {  // narrow tiles: this warp has no chunk, it only releases the accumulator stage
-      tc_fence_before();
-      __syncwarp();
-      if (lane_id() == 0) {
-        if constexpr (CTAS == 2) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty_bar[acc]), 0));
-        else mbar_arrive(&tempty_bar[acc]);
-      }
-    }
 #pragma unroll 1
     for (int c = grp; c < BN / 32; c += NGRP) {
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), r);
-      tmem_ld_wait();
-      if (c + NGRP >= BN / 32) {  // last TMEM read of this warp for this tile: hand the stage back to the MMA warp
-        tc_fence_before();
-        __syncwarp();
-        if (lane_id() == 0) {
-          if constexpr (CTAS == 2) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty_bar[acc]), 0));
-          else mbar_arrive(&tempty_bar[acc]);
-        }
-      }
       const int nb = n0 + c * 32;
       if (nb >= p.N) continue;  // warp-uniform; rows beyond M keep going (their loads are guarded, stores clipped)
       float v[32];
+      {
+        const int tr = q * 32 + (int)lane_id();
 #pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
+        for (int j = 0; j < 32; j += 4) {
+          const float4 a4 = *reinterpret_cast<const float4*>(sacc + acc_idx<BN>(tr, c * 32 + j));
+          v[j] = a4.x; v[j + 1] = a4.y; v[j + 2] = a4.z; v[j + 3] = a4.w;
+        }
+      }
       if (p.alpha != 1.f) {
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[j] *= p.alpha;
@@ -538,18 +482,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_tcgen05(const __gri
     }
     if (p.tma_store && lane_id() == 0) bulk_wait_read0();  // staging buffer must outlive the last bulk store
   }
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CTAS == 2) cluster_sync_all();  // neither CTA may leave while the other's MMAs / TMA still target it
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CTAS == 2) tmem_dealloc_pair(tmem_base, 2 * BN);
-    else tmem_dealloc(tmem_base, 2 * BN);
-  }
 }
-
-#undef ST5_TILE0
-#undef ST5_TILE_STEP
 
 // ---------------------------------------------------------------------------------------------- host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -574,7 +507,7 @@ static int num_sms() {
   if (n == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
@@ -645,17 +578,17 @@ static int make_operand_map(CUtensorMap* map, const void* ptr, int mn_major, int
   return r == CUDA_SUCCESS ? 0 : -12;
 }
 
-template <int BN, int STAGES, bool A_MN, bool B_MN, int CTAS = 1>
+template <int BN, int STAGES, bool A_MN, bool B_MN>
 static int launch_variant(const GemmDesc& g, const EpiParams& ep, cudaStream_t stream) {
-  constexpr int TILE_M = BLOCK_M * CTAS;  // CTAS = 2: one CTA pair per 256 x BN tile, B columns split between the CTAs
   CUtensorMap ma, mb;
   int rc = make_operand_map(&ma, g.A, g.a_mn, g.M, g.K, g.a_ld, g.nb1, g.a_bs1, g.nb2, g.a_bs2, BLOCK_M);
   if (rc) return rc;
-  rc = make_operand_map(&mb, g.B, g.b_mn, g.N, g.K, g.b_ld, g.nb1, g.b_bs1, g.nb2, g.b_bs2, BN / CTAS);
+  rc = make_operand_map(&mb, g.B, g.b_mn, g.N, g.K, g.b_ld, g.nb1, g.b_bs1, g.nb2, g.b_bs2, BN);
   if (rc) return rc - 10;
-  constexpr size_t smem = (size_t)STAGES * (BLOCK_M * BLOCK_K * 2 + (BN / CTAS) * BLOCK_K * 2) + EPI_WARPS * 4096 +
-                          (2 * STAGES + 4) * 8 + 16 + 1024;
-  auto kern = gemm_bf16_tcgen05<BN, STAGES, A_MN, B_MN, CTAS>;
+  constexpr size_t smem = (size_t)STAGES * (BLOCK_M * BLOCK_K * 2 + BN * BLOCK_K * 2) + BLOCK_M * BN * 4 +
+                          EPI_WARPS * 4096 + 2 * STAGES * 8 + 1024;
+  static_assert(smem <= 227 * 1024, "GEMM tile does not fit the 227 KB of shared memory of a block");
+  auto kern = gemm_bf16_wgmma<BN, STAGES, A_MN, B_MN>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -663,7 +596,7 @@ static int launch_variant(const GemmDesc& g, const EpiParams& ep, cudaStream_t s
     attr_set = true;
   }
   EpiParams e2 = ep;
-  e2.tiles_m = (g.M + TILE_M - 1) / TILE_M;
+  e2.tiles_m = (g.M + BLOCK_M - 1) / BLOCK_M;
   e2.tiles_n = (g.N + BN - 1) / BN;
   const long total = (long)e2.tiles_m * e2.tiles_n * g.nb1 * g.nb2;
   if (total > 0x7fffffffL) return -4;
@@ -694,8 +627,8 @@ static int launch_variant(const GemmDesc& g, const EpiParams& ep, cudaStream_t s
   if (e2.act == ACT_GELU_TANH_GATE &&
       (!e2.tma_store || g.c_fp32 || g.C_pre == nullptr || (g.N & 7) != 0 || g.residual != nullptr || g.ag_pre != nullptr))
     return -5;  // the gate epilogue needs the TMA-store layout, bf16 outputs and an 8-aligned row length
-  const long slots = num_sms() / CTAS;
-  const int grid = (int)(total < slots ? total : slots) * CTAS;  // one persistent CTA (or CTA pair per TPC) per SM
+  const long slots = num_sms();
+  const int grid = (int)(total < slots ? total : slots);  // one persistent CTA per SM
   static const bool pdl = [] {
     const char* e = getenv("ST5_PDL");
     return e == nullptr || atoi(e) != 0;
@@ -705,15 +638,8 @@ static int launch_variant(const GemmDesc& g, const EpiParams& ep, cudaStream_t s
   cfg.blockDim = dim3(GEMM_THREADS);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   int na = 0;
-  if (CTAS == 2) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = 2;
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
   if (pdl) {
     attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[na].val.programmaticStreamSerializationAllowed = 1;
@@ -726,14 +652,14 @@ static int launch_variant(const GemmDesc& g, const EpiParams& ep, cudaStream_t s
   return (int)cudaGetLastError();
 }
 
-template <int BN, int STAGES, int CTAS = 1>
+template <int BN, int STAGES>
 static int launch_major(const GemmDesc& g, const EpiParams& ep, cudaStream_t stream) {
   if (g.a_mn) {
-    if (g.b_mn) return launch_variant<BN, STAGES, true, true, CTAS>(g, ep, stream);
-    return launch_variant<BN, STAGES, true, false, CTAS>(g, ep, stream);
+    if (g.b_mn) return launch_variant<BN, STAGES, true, true>(g, ep, stream);
+    return launch_variant<BN, STAGES, true, false>(g, ep, stream);
   }
-  if (g.b_mn) return launch_variant<BN, STAGES, false, true, CTAS>(g, ep, stream);
-  return launch_variant<BN, STAGES, false, false, CTAS>(g, ep, stream);
+  if (g.b_mn) return launch_variant<BN, STAGES, false, true>(g, ep, stream);
+  return launch_variant<BN, STAGES, false, false>(g, ep, stream);
 }
 
 int gemm_launch(const GemmDesc& g, cudaStream_t stream) {
@@ -756,8 +682,8 @@ int gemm_launch(const GemmDesc& g, cudaStream_t stream) {
   ep.a_m1 = (g.nb1 > 1 && g.a_bs1 == 0) ? 0 : 1; ep.a_m2 = (g.nb2 > 1 && g.a_bs2 == 0) ? 0 : 1;
   ep.b_m1 = (g.nb1 > 1 && g.b_bs1 == 0) ? 0 : 1; ep.b_m2 = (g.nb2 > 1 && g.b_bs2 == 0) ? 0 : 1;
   ep.c_m1 = (g.nb1 > 1 && g.c_bs1 == 0) ? 0 : 1; ep.c_m2 = (g.nb2 > 1 && g.c_bs2 == 0) ? 0 : 1;
-  // Tile width: minimise (rounds of the persistent grid) x (time per tile). A 128x256 tile reads 12 KB of smem per
-  // 128-cycle MMA (under the 128 B/clk port); 128x128 and 128x64 tiles are smem-port bound, hence the >1 factors.
+  // Tile width: minimise (rounds of the persistent grid) x (time per tile); a 128 x 64 tile moves more operand bytes
+  // per FLOP than a 128 x 128 one, hence its > 1 factor.
   const long tiles_m = (g.M + BLOCK_M - 1) / BLOCK_M;
   const long batch = (long)g.nb1 * g.nb2;
   const long sms = num_sms();
@@ -766,39 +692,15 @@ int gemm_launch(const GemmDesc& g, cudaStream_t stream) {
     const long rounds = (tiles + sms - 1) / sms;
     return (double)rounds * (bn * factor + 24.0);
   };
-  static const int force_bn = [] {  // tuning / profiling knob: ST5_GEMM_BN=64|128|256 pins the tile width
+  static const int force_bn = [] {  // tuning / profiling knob: ST5_GEMM_BN=64|128 pins the tile width
     const char* e = getenv("ST5_GEMM_BN");
     return e ? atoi(e) : 0;
   }();
-  // ST5_GEMM_PAIR=1|2 (experimental, off by default until measured on the GPU; 2 = 5-stage ring): 256 x 256 tiles on CTA pairs for every
-  // problem the 256-wide tile would have been chosen for and that has at least one full pair of row blocks.
-  static const int pair_mode = [] {
-    const char* e = getenv("ST5_GEMM_PAIR");
-    return e ? atoi(e) : -1;  // -1 = automatic (measured rule below), 0 = never, 1 / 2 = wherever the 256-wide tile applies
-  }();
-  if (force_bn == 256) return launch_major<256, 3>(g, ep, stream);
-  if (force_bn == 128) return launch_major<128, 5>(g, ep, stream);
+  if (force_bn == 128) return launch_major<128, 4>(g, ep, stream);
   if (force_bn == 64) return launch_major<64, 6>(g, ep, stream);
-  const double c256 = g.N > 128 ? cost(256, 1.0) : 1e30;
-  const double c128 = g.N > 64 ? cost(128, 1.12) : 1e30;
-  const double c64 = cost(64, 1.35);
-  // Weight gradients (accumulate == 2: both operands MN-major, long contraction split over the batch dimension by the
-  // caller so that the CTA pairs fill the machine): 256 x 256 pair tiles halve the operand bytes per FLOP, which is what
-  // bounds these GEMMs (128 x 128 tiles: 36 % tensor-pipe activity, the library reaches 1.45 PFLOP/s on the same shapes)
-  if (pair_mode != 0 && force_bn == 0 && g.accumulate == 2 && g.M >= 2 * BLOCK_M && g.N >= 192)
-    return launch_major<256, 4, 2>(g, ep, stream);
-  if (c256 <= c128 && c256 <= c64) {
-    if (pair_mode == 2 && g.M > BLOCK_M) return launch_major<256, 5, 2>(g, ep, stream);  // deeper ring (tuning)
-    if (pair_mode == 1 && g.M > BLOCK_M) return launch_major<256, 4, 2>(g, ep, stream);
-    // Automatic: the CTA pair wins where operand feed is the limit and there are several rounds of tiles (measured on a
-    // B200, profiles/r02_pair_gemm_check.log: 8192^3 x1.15, M=10016 N=3072 K=768 x1.18, K=3072 x1.04), loses on
-    // single-round grids and on the two-output GELU epilogue (x0.89-0.97).
-    if (pair_mode == -1 && g.M >= 4096 && !g.a_mn && batch == 1 && g.C_pre == nullptr &&
-        ((long)g.K >= 3072 || ((long)g.N >= 3072 && (long)g.M >= 8192) || (g.ag_pre != nullptr && (long)g.N >= 3072)))
-      return launch_major<256, 4, 2>(g, ep, stream);
-    return launch_major<256, 3>(g, ep, stream);
-  }
-  if (c128 <= c64) return launch_major<128, 5>(g, ep, stream);
+  const double c128 = g.N > 64 ? cost(128, 1.0) : 1e30;
+  const double c64 = cost(64, 1.25);
+  if (c128 <= c64) return launch_major<128, 4>(g, ep, stream);
   return launch_major<64, 6>(g, ep, stream);
 }
 

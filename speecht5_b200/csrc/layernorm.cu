@@ -206,11 +206,8 @@ __global__ void __launch_bounds__(256)
 // bias gradient of the projection that produced x: its separate column-sum launch disappears) -- live in a PRIVATE
 // shared-memory strip per warp (plain read-modify-write of the lane's own 16-byte slots, conflict-free layout), which
 // frees the registers for a one-row-ahead prefetch of dy / s: a warp visits only 2-5 rows, so without the prefetch every
-// row costs a full exposed HBM round trip (measured 2.5 TB/s before, 3.1 TB/s with it; what bounds it now is bytes in
-// flight: 16 warps x 3 KB per SM. A three-CTA form that kept the rows packed in registers and decoded them twice was
-// measured at 2.2 TB/s -- spills and the doubled decode cost more than the third CTA's loads bought -- and so did a
-// form that staged three rows per warp through a cp.async ring with ONE strip per CTA (shared-memory fp32 atomics):
-// 2.2 TB/s, the 72 atomics per row and lane cost more than the extra bytes in flight bought. Both removed.) The strips meet after a CTA barrier and leave as
+// row costs a full exposed HBM round trip; what bounds it then is bytes in flight: 16 warps x 3 KB per SM. The strips
+// meet after a CTA barrier and leave as
 // 16-byte vector reductions (red.global.add.v4.f32) when the targets are 16-byte aligned. NCH = 16-byte chunks per lane.
 constexpr int LNB_WARPS = 8;
 constexpr int LNB_NACC = 3;  // dgamma | dbeta | column sums of dx

@@ -257,10 +257,10 @@ int bn_fwd_launch(const void* x, int64_t x_ld, const float* gamma, const float* 
   const float ds = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
   const int64_t n = rows * C;
   int64_t g = (n + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   if (bn_vec_ok(C, {x_ld, y_ld}, {x, y, y_pre, gamma, beta, save_mean, save_rstd})) {
     int64_t gv = (n / 8 + 255) / 256;
-    if (gv > 148 * 16) gv = 148 * 16;
+    if (gv > 132 * 16) gv = 132 * 16;
     if (dtype == ST5_F32)
       bn_apply_vec_kernel<float><<<(unsigned)gv, 256, 0, s>>>((const float*)x, x_ld, gamma, beta, save_mean, save_rstd,
                                                               (float*)y, y_ld, (float*)y_pre, rows, (int)C, act, thr,
@@ -368,7 +368,7 @@ int bn_bwd_launch(const void* dy, int64_t dy_ld, const void* x, int64_t x_ld, co
   dim3 grid((unsigned)((C + 31) / 32), (unsigned)nb), block(32, 8);
   const int64_t n = rows * C;
   int64_t g = (n + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   if (bn_vec_ok(C, {dy_ld, x_ld, dx_ld}, {dy, x, y_pre, dx, gamma, save_mean, save_rstd, scratch})) {
     // (each block covers 256 channels: split the rows finer than the scalar kernel to keep ~4 blocks per SM busy)
     const int64_t cblocks = (C + 255) / 256;
@@ -378,7 +378,7 @@ int bn_bwd_launch(const void* dy, int64_t dy_ld, const void* x, int64_t x_ld, co
     rpb = (rows + vnb - 1) / vnb;
     dim3 vgrid((unsigned)cblocks, (unsigned)((rows + rpb - 1) / rpb));
     int64_t gv = (n / 8 + 255) / 256;
-    if (gv > 148 * 16) gv = 148 * 16;
+    if (gv > 132 * 16) gv = 132 * 16;
     if (dtype == ST5_F32) {
       bn_bwd_stat_vec_kernel<float><<<vgrid, block, 0, s>>>((const float*)dy, dy_ld, (const float*)x, x_ld,
                                                             (const float*)y_pre, save_mean, save_rstd, scratch, rows,

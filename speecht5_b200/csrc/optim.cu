@@ -31,7 +31,7 @@ int sumsq_launch(const float* x, int64_t n, float* out, cudaStream_t s) {
   if (n == 0) return 0;
   if (reinterpret_cast<uintptr_t>(x) & 15) return -2;
   int64_t g = (n / 4 + 255) / 256;
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > 132 * 8) g = 132 * 8;
   if (g < 1) g = 1;
   launch_pdl(sumsq_kernel, dim3((unsigned)g), dim3(256), 0, s, x, n, out);
   return (int)cudaGetLastError();
@@ -107,7 +107,7 @@ int adam_launch(float* p, const float* g, float* m, float* v, void* p_bf16, int6
     step_size = (float)((lr_dev != nullptr ? 1.0 : (double)lr) * sqrt(bc2) / bc1);
   }
   int64_t gsz = (n + 255) / 256;
-  if (gsz > 148 * 16) gsz = 148 * 16;
+  if (gsz > 132 * 16) gsz = 132 * 16;
   launch_pdl(adam_kernel, dim3((unsigned)gsz), dim3(256), 0, s, p, g, m, v, (__nv_bfloat16*)p_bf16, n, lr, beta1, beta2, eps, weight_decay, step_size, grad_norm_sq, max_norm, grad_mul, lr_dev, step_dev);
   return (int)cudaGetLastError();
 }

@@ -14,7 +14,7 @@ Device formulation (channels-last activations [B, T, C] throughout, no im2col, n
   warp per frame (kernels.conv0_ln_gelu_fwd / _bwd);
 * layers 1..6 in "layer_norm" mode: the same window GEMM without an epilogue activation, the row LayerNorm kernel of
   the transformer blocks (ops.residual_layer_norm, fp32 statistics) and a stand-alone GELU (kernels.act_fwd / act_bwd);
-* layers 1..6 forward: ONE batched tcgen05 GEMM each over an overlapping-window view of the input -- row t of
+* layers 1..6 forward: ONE batched wgmma GEMM each over an overlapping-window view of the input -- row t of
   utterance b is the k*C_in contiguous elements starting at frame t*stride (row pitch stride*C_in) -- with GELU and
   the pre-activation store in the epilogue;
 * input gradient: the transposed convolution split by output phase r = i mod stride; phase r is a window GEMM over

@@ -13,9 +13,9 @@ class GreedyGenerator:
                  len_penalty=1.0, unk_penalty=0.0, temperature=1.0, ctc_weight=0.0, lm_model=None, use_cache=True,
                  blank=None, mask_idx=None, **unused):
         if beam_size != 1:
-            raise NotImplementedError("beam search > 1 is not built in the B200 path (SURVEY section 2): use --beam 1")
+            raise NotImplementedError("beam search > 1 is not built in the H100 path (SURVEY section 2): use --beam 1")
         if ctc_weight and ctc_weight > 0 or lm_model is not None:
-            raise NotImplementedError("CTC rescoring / LM fusion are not built in the B200 path")
+            raise NotImplementedError("CTC rescoring / LM fusion are not built in the H100 path")
         self.model = models[0] if isinstance(models, (list, tuple)) else models
         self.tgt_dict = tgt_dict
         self.pad, self.eos, self.unk = tgt_dict.pad(), tgt_dict.eos(), tgt_dict.unk()

@@ -20,7 +20,7 @@ def _act_dtype(x):
 
 
 def _attend(*a, **kw):
-    """One-row queries: the row kernels (the fused tcgen05 path works on 128-query tiles)."""
+    """One-row queries: the row kernels (the fused wgmma path works on 64-query tiles)."""
     prev = RT.attn_tensor_core
     RT.attn_tensor_core = False
     try:

@@ -1,4 +1,4 @@
-"""Shared Transformer encoder / decoder of SpeechT5 on the B200 kernel library.
+"""Shared Transformer encoder / decoder of SpeechT5 on the H100 kernel library.
 
 Host-side mirror of the reference modules -- same class names, constructor arguments, parameter names and return
 contracts -- with every tensor op routed to libspeecht5_b200.so through speecht5_b200.ops:
@@ -45,7 +45,7 @@ class MultiheadAttention(nn.Module):
         self.dropout_p = dropout
         self.head_dim = embed_dim // num_heads
         assert self.head_dim * num_heads == embed_dim, "embed_dim must be divisible by num_heads"
-        assert self.head_dim == 64, "the B200 attention kernels are specialised for head_dim 64 (Base and Large)"
+        assert self.head_dim == 64, "the attention kernels are specialised for head_dim 64 (Base and Large)"
         self.scaling = self.head_dim ** -0.5
         self.self_attention = self_attention
         self.encoder_decoder_attention = encoder_decoder_attention

@@ -1,4 +1,4 @@
-"""`t5_transformer` model and its architecture presets on the B200 kernel library -- drop-in for
+"""`t5_transformer` model and its architecture presets on the H100 kernel library -- drop-in for
 speecht5/models/speecht5.py (reference): same registry names (@register_model "t5_transformer"; archs t5_transformer,
 t5_transformer_base, t5_transformer_large, t5_transformer_base_asr :1252,1385,1402,1427), same forward signature
 (:786) and return tuples, same parameter names (checkpoints load with load_state_dict).
@@ -281,7 +281,7 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
                                       "(task with HuBERT label dictionaries, or --hubert-num-classes)")
         if not built:
             raise NotImplementedError(
-                f"T5TransformerModel.forward: {input_type}->{output_type} (task {task_name}) is not built in the B200 "
+                f"T5TransformerModel.forward: {input_type}->{output_type} (task {task_name}) is not built in the H100 "
                 "path (speaker identification / voice conversion / enhancement branches)")
         features_pen = frame_mask_indices = None
         if speech_in and target_list is not None:  # (:813-815) speech pre-training: frames aligned with the labels
@@ -361,7 +361,7 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
         filtered = {k: v for k, v in state_dict.items() if k in own and own[k].shape == v.shape}
         dropped = [k for k in state_dict if k not in filtered]
         if dropped:
-            logger.info("load_state_dict: ignoring %d keys absent/mismatched in the B200 t2s model", len(dropped))
+            logger.info("load_state_dict: ignoring %d keys absent/mismatched in the H100 t2s model", len(dropped))
         out = super().load_state_dict(filtered, strict=False)
         RT.params_written_externally()  # incl. the trainer's flat bf16 shadow, if one exists (fairseq: build, then load)
         return out

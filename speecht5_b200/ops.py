@@ -4,7 +4,7 @@ backward computation below is a call into the hand-written CUDA library (speecht
 Two numeric modes (Runtime.dtype):
   * torch.bfloat16 -- throughput mode: bf16 activations, bf16 tensor-core GEMMs with fp32 accumulation, fp32 statistics.
   * torch.float32  -- parity mode: fp32 activations; each GEMM is evaluated as hi*hi + hi*lo + lo*hi over bf16 splits of
-    both operands (three accumulate passes of the same tcgen05 kernel), i.e. ~2^-16 relative operand error.
+    both operands (three accumulate passes of the same wgmma kernel), i.e. ~2^-16 relative operand error.
 """
 import os
 
@@ -30,8 +30,8 @@ class Runtime:
         self._static_grad = {}  # key -> fp32 view of the trainer's flat gradient buffer (direct accumulation)
         self._static_refresh = None  # callable that re-casts the owner's flat bf16 shadow from its fp32 master
         self._static_dirty = False   # fp32 parameters were written behind the owner's back (load_state_dict)
-        self.attn_tensor_core = True  # bf16 mode: contractions of attention on the tcgen05 GEMM (else row kernels)
-        self.attn_fused = True        # bf16 mode, no RPE, Tk <= 320: single-launch fused forward (attention_fused.cu)
+        self.attn_tensor_core = True  # bf16 mode: contractions of attention on the wgmma GEMM (else row kernels)
+        self.attn_fused = True        # bf16 mode, Tk <= 320: single-launch fused forward (attention_flash.cu)
         self.attn_fused_bwd = True    # ... and the flash-style fused backward (attention_fused_bwd.cu)
         self.fold_residual_grad = os.environ.get("ST5_FOLD_RESGRAD", "1") != "0"  # see LinearFn.forward (passthrough)
         self.probs_grad_heads = 0     # > 0: gradients on returned probabilities exist for the first n heads only
@@ -40,7 +40,7 @@ class Runtime:
         # every bf16 shape goes through it (ST5_ATTN_FLASH=all)
         self.attn_flash = {"0": False, "all": "all"}.get(os.environ.get("ST5_ATTN_FLASH", "1"), True)
         self.ffn_gate = os.environ.get("ST5_FFN_GATE", "1") != "0"  # bf16 mode: fc1 stores the backward gate (FFNFn)
-        self.wgrad_splitk = os.environ.get("ST5_WGRAD_SPLITK", "1") != "0"  # weight gradients: pair tiles + split-K + L2 reduce
+        self.wgrad_splitk = os.environ.get("ST5_WGRAD_SPLITK", "1") != "0"  # weight gradients: split-K + L2 reduce
         # out_proj / fc2 bias gradients come out of the consuming LayerNorm's backward pass (no column-sum launch)
         self.fold_bias_grad = os.environ.get("ST5_FOLD_BIAS_GRAD", "1") != "0"
         self.fp32_stream = os.environ.get("ST5_FP32_STREAM", "1") != "0"  # bf16 mode: fp32 residual stream between LayerNorms
@@ -253,7 +253,7 @@ def wgrad_mm(gy, gy_ld, xin, xin_ld, n_out, n_in, M, target=None):
                  and n_in >= 192 and target.is_contiguous() and target.data_ptr() % 16 == 0 and n_in % 4 == 0)
     if not splitk_l2 and gy[1] is None and xin[1] is None and tiles <= 72 and M >= 2048:
         for cand in (8, 6, 4, 3, 2):
-            if cand * tiles <= 320 and M % cand == 0:
+            if cand * tiles <= 2 * 132 and M % cand == 0:  # at most two waves of 128 x 128 tiles
                 S = cand
                 break
     if S > 1:
@@ -265,14 +265,13 @@ def wgrad_mm(gy, gy_ld, xin, xin_ld, n_out, n_in, M, target=None):
         K.colsum(parts.view(S, n_out * n_in), out.view(-1), accumulate=target is not None)
         return None if target is not None else out
     if splitk_l2:
-        # throughput mode, straight into the flat gradient buffer: 256 x 256 CTA-pair tiles, the contraction split over
-        # the batch dimension so that (tiles x splits) fills the 74 pairs of the chip, every partial product added to
-        # the gradient by a TMA reduce at the L2 (nobody reads the gradient first, no partial buffers, no reduction
-        # launch). Splits must divide M: a batch entry is a [chunk]-row window of the MN-major operands.
-        tp = ((n_out + 255) // 256) * ((n_in + 255) // 256)
+        # throughput mode, straight into the flat gradient buffer: the contraction split over the batch dimension so
+        # that (128 x 128 tiles x splits) fills one wave of the 132 SMs, every partial product added to the gradient by
+        # a TMA reduce at the L2 (nobody reads the gradient first, no partial buffers, no reduction launch). Splits
+        # must divide M: a batch entry is a [chunk]-row window of the MN-major operands.
         S = 1
         for cand in (16, 12, 10, 8, 6, 5, 4, 3, 2):
-            if cand * tp <= 76 and M % cand == 0 and M // cand >= 512:
+            if cand * tiles <= 132 and M % cand == 0 and M // cand >= 512:
                 S = cand
                 break
         chunk = M // S
@@ -785,13 +784,13 @@ class AttentionFn(torch.autograd.Function):
 
 class AttentionTCFn(torch.autograd.Function):
     """bf16 tensor-core attention: every contraction (QK^T, Q.PE^T, PV and the five backward products) is a batched
-    launch of the tcgen05 GEMM over (head, utterance) reading q/k/v in place from the fused projection buffers; the
+    launch of the wgmma GEMM over (head, utterance) reading q/k/v in place from the fused projection buffers; the
     softmax / dS / relative-position scatter steps are the row kernels of csrc/attention_tc.cu. Same interface and
     dropout-mask convention as AttentionFn (the exact fp32 row-kernel path used for parity mode)."""
 
     @staticmethod
     def _fused_backward(q_buf, kv_buf, probs, cfg, off, seed, p_ld, same, fused, dout, dprobs):
-        """One launch (+ the row-constant pre-pass): flash-style backward on tcgen05 (attention_fused_bwd.cu). `fused` =
+        """One launch (+ the row-constant pre-pass): flash-style backward on wgmma (attention_fused_bwd.cu). `fused` =
         (out, psave, inv_l, key_pad): psave / inv_l are the exponentials (dropout decision in the sign bit) and the row
         normalisers the forward saved; `probs` the fp32 probabilities it returned to the caller (only with dprobs)."""
         out, psave, inv_l, o32, kp = fused
@@ -921,14 +920,14 @@ class AttentionTCFn(torch.autograd.Function):
         causal = bool(cfg.get("causal", False))
         rpe_fused = (pe_k is not None and use_fused and not causal and 0 < maxpos <= 160
                      and Tq <= maxpos and Tk <= maxpos and pe_k.shape[0] == 2 * maxpos)
-        resident = rpe_fused or (pe_k is None and Tk <= 320 and use_fused)  # whole score rows fit TMEM: one launch
+        resident = rpe_fused or (pe_k is None and Tk <= 320 and use_fused)  # bounded score rows: one launch
         # streaming kernel (attention_flash.cu): any length, clipped relative positions; RT.attn_flash == "all" also
         # routes the shapes the resident kernel could take through it
         flash = (use_fused and RT.attn_flash and (pe_k is None or (not causal and maxpos > 0 and pe_k.shape[0] == 2 * maxpos))
                  and (not resident or RT.attn_flash == "all"))
         if resident or flash:
-            # ONE launch: QK^T (+ the relative-position bias gathered on chip from QP = Q PE^T in TMEM) -> masks ->
-            # softmax -> dropout -> PV with the scores resident in TMEM. For the backward pass the kernel saves the
+            # ONE launch: QK^T (+ the relative-position bias gathered on chip from QP = Q PE^T) -> masks ->
+            # softmax -> dropout -> PV with the scores on chip. For the backward pass the kernel saves the
             # exponentials (bf16, dropout decision in the sign bit) and 1/rowsum; normalised fp32 probabilities are
             # written only when the caller asked for them (need_head_weights)
             drop_p = cfg.get("drop_p", 0.0)
@@ -1076,10 +1075,10 @@ def attention(q_buf, kv_buf, *, H, d, q_col, k_col, v_col, scale, pe_k=None, max
 # =================================================================================================== postnet blocks
 def _conv_wgrad_split(Cout, Ncols, Kd):
     """Split of the post-net weight-gradient contraction (K = all frames of the batch, ~20 k) over the GEMM's batch
-    dimension: (S, chunk) with S * chunk >= Kd, chunk a multiple of 8 rows. The output has a handful of tiles only, so
-    without the split 5 - 20 CTAs do all the work (83 us per conv; the library needs 19)."""
-    tiles = ((Cout + 255) // 256 if Cout >= 256 else (Cout + 127) // 128) * ((Ncols + 255) // 256)
-    S = max(1, min(32, 148 // max(1, tiles) if Cout < 256 else 74 // max(1, tiles), Kd // 512))
+    dimension: (S, chunk) with S * chunk >= Kd, chunk a multiple of 8 rows. The output has a handful of 128 x 128 tiles
+    only, so without the split a few CTAs would do all the work; S fills one wave of the 132 SMs."""
+    tiles = ((Cout + 127) // 128) * ((Ncols + 127) // 128)
+    S = max(1, min(32, 132 // max(1, tiles), Kd // 512))
     chunk = ((Kd + S - 1) // S + 7) // 8 * 8
     return S, chunk
 

@@ -4,7 +4,7 @@
 projection, time-first input) and the code mixing of models/speecht5.py:858-872.
 
 Used by the speech pre-training branch of T5TransformerModel.forward (target_list / --use-codebook); the criteria
-are criterions/speech_pretrain_criterion.py and text_pretrain_criterion.py. The two projections run on the tcgen05 GEMM
+are criterions/speech_pretrain_criterion.py and text_pretrain_criterion.py. The two projections run on the wgmma GEMM
 (ops.linear); the rest acts on [frames, classes]-sized tensors (cosine similarities against the label embeddings,
 Gumbel-softmax over 100 variables, a 200 x d codebook product) and is issued as torch calls. Checked on the CPU against
 oracle/pretrain_oracle.py through the kernel emulation (tests/test_frontend_cpu.py), forward and backward.

@@ -3,7 +3,7 @@
 Mirrors what fairseq does around the model for one update -- fairseq/trainer.py:675-952 (zero_grad -> per-micro-batch
 task.train_step -> all_reduce_grads -> multiply_grads(world / sample_size) -> clip_grad_norm -> optimizer.step) with
 LegacyDistributedDataParallel semantics for the gradient exchange (legacy_distributed_data_parallel.py:76-165: grads
-/= world, all-reduce(sum), parameters without a gradient contribute zeros) -- re-designed for B200:
+/= world, all-reduce(sum), parameters without a gradient contribute zeros) -- re-designed for H100:
 
   * parameters, gradients, Adam moments live in single flat fp32 buffers plus a flat bf16 shadow; fused operand groups
     (q|k|v weights, k|v, feat_out|prob_out, and their biases) are laid out adjacently so the GEMMs read them in place;
@@ -233,8 +233,7 @@ class B200Trainer:
             raise ValueError("parity mode reads the fp32 masters in every GEMM: use exchange='allreduce'")
         self.exchange = exchange if self.world > 1 else "none"
         # layers per exchange stage: fewer, larger collectives (each NCCL launch has to squeeze its CTAs in between
-        # persistent 148-CTA GEMM grids) against later overlap; ST5_STAGE_GROUP overrides. Measured at N=2 (weak scaling
-        # efficiency, profiles/r02_n2_exchange.txt): 1 layer per stage 0.960, 3 -> 0.972, 6 -> 0.975, no overlap 0.935
+        # persistent 132-CTA GEMM grids) against later overlap; ST5_STAGE_GROUP overrides
         self.stage_group = int(os.environ.get("ST5_STAGE_GROUP", stage_group))
         self.fp = FlatParams(model, self.world if self.exchange == "shard" else 1, self.rank, self.stage_group)
         self.bucketer = GradBucketer(self.fp.grads, bucket_elems=bucket_mb * 1024 * 1024 // 4, group=process_group)

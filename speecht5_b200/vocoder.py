@@ -2,7 +2,7 @@
 tree's SpeechUT/fairseq/fairseq/models/text_to_speech/hifigan.py:13-170 with the SpeechT5 vocoder configuration).
 
 Every convolution is a window GEMM on the existing
-tcgen05 kernel over channels-last activations (no im2col); the operand views are checked on the CPU through the GEMM
+wgmma kernel over channels-last activations (no im2col); the operand views are checked on the CPU through the GEMM
 emulator against oracle/audio_oracle.py:HifiGanGenerator (tests/test_frontend_cpu.py).
 
 * Conv1d(k, padding (k-1)/2): one batched GEMM over the zero-padded input, row t = the k*C contiguous elements from

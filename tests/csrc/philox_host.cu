@@ -68,10 +68,10 @@ int main() {
     const Philox4 r = philox4x32(1, 2, 3);
     std::printf("kat %08x %08x %08x %08x\n", r.x, r.y, r.z, r.w);
     std::printf("pitch %llu %llu\n", (unsigned long long)attn_drop_pitch(313), (unsigned long long)attn_drop_pitch(160));
-    // tcgen05 instruction descriptors (kind::f16, bf16 x bf16 -> fp32): c_format bit 4, a/b formats bits 7/10, a/b major
-    // bits 15/16, N >> 3 at bit 17, M >> 4 at bit 24
-    std::printf("idesc %08x %08x %08x\n", umma_idesc_bf16(128, 256, 0, 0), umma_idesc_bf16(128, 64, 1, 1),
-                umma_idesc_bf16(128, 160, 0, 1));
+    // wgmma shared-memory descriptors (16-byte units): start address bit 0, leading byte offset bit 16, stride byte
+    // offset bit 32, 128B swizzle = layout type 1 at bit 62
+    std::printf("desc %016llx %016llx\n", (unsigned long long)wgmma_smem_desc(0x1000, 16, 1024),
+                (unsigned long long)wgmma_smem_desc(0x2040, 8192, 1024));
   }
   return 0;
 }

@@ -113,18 +113,17 @@ def test_argument_errors_are_reported_without_touching_a_device(lib):
 
 def test_register_budget_of_the_wide_kernels(lib):
     """A launch fails with 'too many resources requested' when registers x allocated warps exceed the 64 K file. Warps
-    are allocated four at a time, so an 18-warp block (576 threads: the tcgen05 GEMM, both fused attention kernels)
-    pays for 20: 96 registers per thread is the ceiling. (A 112-register build once passed every CPU check and failed
-    every launch on the GPU; ptxas does not know the block size unless __launch_bounds__ says so.)"""
+    are allocated four at a time, so a 9-warp block (288 threads: both attention kernels) pays for 12 and the 12-warp
+    GEMM block for 12: 168 registers per thread is the ceiling. (A build over the ceiling passes every CPU check and
+    fails every launch on the GPU; ptxas does not know the block size unless __launch_bounds__ says so.)"""
     import shutil
     import subprocess
     from speecht5_b200.build import LIB
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not available")
     out = subprocess.run(["cuobjdump", "-res-usage", LIB], capture_output=True, text=True).stdout
-    threads = {"gemm_bf16_tcgen05": (576, 1), "attn_fused_bwd_kernel": (576, 1), "attn_fused_fwd_kernelILb0": (576, 1),
-               "attn_fused_fwd_kernelILb1": (320, 1), "attn_flash_fwd_kernelILb1": (320, 1),
-               "attn_flash_fwd_kernelILb0": (384, 2)}  # (threads per block, blocks that must fit one SM)
+    threads = {"gemm_bf16_wgmma": (384, 1), "attn_fused_bwd_kernel": (288, 1), "attn_flash_fwd_kernelILb1": (288, 1),
+               "attn_flash_fwd_kernelILb0": (288, 1)}  # (threads per block, blocks that must fit one SM)
     seen = 0
     for m in re.finditer(r"Function (\S+):\s*\n\s*REG:(\d+)", out):
         name, regs = m.group(1), int(m.group(2))

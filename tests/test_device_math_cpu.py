@@ -25,7 +25,7 @@ def stats(tmp_path_factory):
     for line in out.splitlines():
         parts = line.split()
         res[" ".join(parts[:-1]) if parts[0] == "keep_rate" else parts[0]] = parts[1:] \
-            if parts[0] in ("kat", "pitch", "idesc") else float(parts[-1])
+            if parts[0] in ("kat", "pitch", "desc") else float(parts[-1])
     return res
 
 
@@ -46,10 +46,10 @@ def test_known_answers(stats):
     any checkpointed seed, depend on it."""
     assert stats["kat"] == ["15da0e38", "90b50218", "61766a43", "4b911f60"]
     assert stats["pitch"] == ["320", "160"]
-    # instruction descriptors: (1<<4)|(1<<7)|(1<<10) | a_mn<<15 | b_mn<<16 | (N>>3)<<17 | (M>>4)<<24
-    base = (1 << 4) | (1 << 7) | (1 << 10) | ((128 >> 4) << 24)
-    want = [base | ((256 >> 3) << 17), base | (1 << 15) | (1 << 16) | ((64 >> 3) << 17), base | (1 << 16) | ((160 >> 3) << 17)]
-    assert [int(v, 16) for v in stats["idesc"]] == want
+    # shared-memory matrix descriptors: addr>>4 | (lbo>>4)<<16 | (sbo>>4)<<32 | 1<<62 (128B swizzle)
+    want = [(0x1000 >> 4) | ((16 >> 4) << 16) | ((1024 >> 4) << 32) | (1 << 62),
+            (0x2040 >> 4) | ((8192 >> 4) << 16) | ((1024 >> 4) << 32) | (1 << 62)]
+    assert [int(v, 16) for v in stats["desc"]] == want
 
 
 def test_gelu_formulas_meet_their_documented_error_bounds():

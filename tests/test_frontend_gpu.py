@@ -1,6 +1,5 @@
 """-m gpu: the speech-input front end (speecht5_b200/frontend.py + csrc/conv_frontend.cu), CE + CTC criterion, greedy
-decoding, KV cache, log-mel, HiFi-GAN and the pre-training extras against the oracles (first green run on a B200:
-round 2, gpurun_out/r2_first/gated_frontend.log; the opt-in gate of round 1 is gone)."""
+decoding, KV cache, log-mel, HiFi-GAN and the pre-training extras against the oracles."""
 import os
 
 import pytest
@@ -132,7 +131,7 @@ def test_speech_to_text_step_against_the_oracle(cuda, dtype):
 
 
 def test_logmel_on_device_against_the_oracle(cuda):
-    """speecht5_b200/audio.py (STFT and mel projection on the tcgen05 GEMM, split precision) vs oracle/audio_oracle.py."""
+    """speecht5_b200/audio.py (STFT and mel projection on the wgmma GEMM, split precision) vs oracle/audio_oracle.py."""
     import numpy as np
     from oracle.audio_oracle import logmelfilterbank as ref_fn
     from speecht5_b200 import audio

@@ -1,13 +1,13 @@
-"""Pins the oracle restatements against the REFERENCE'S OWN CODE.
+"""Pins the oracle restatements and the plugin against the REFERENCE'S OWN CODE.
 
-Two layers:
-* fixtures `tests/golden/ref_*.npz` were produced by `/root/reference/SpeechT5/speecht5/**` itself (unmodified, loaded by
-  `oracle/ref_loader.py`; generator `tests/golden/make_golden_from_ref.py`): weights, inputs, outputs, the reference
-  criterions' loss terms, gradients, its SequenceGenerator's token ids, its compute_mask_indices draws. The oracle is
-  replayed on the stored weights + inputs and must agree to fp32 round-off (tolerances in each test). These run
-  everywhere (no reference tree needed).
-* when the reference tree is mounted (build container), the fixtures are regenerated in memory and must be identical to
-  the committed ones (stale-fixture guard), and the reference runs at real width / long sequences against the oracle.
+* fixtures `tests/golden/ref_*.npz` were produced by the reference's `SpeechT5/speecht5/**` itself (unmodified, loaded by
+  `oracle/ref_loader.py`; generators `tests/golden/make_golden_from_ref.py`, `make_golden_ref_criteria.py`,
+  `make_golden_ref_pins.py`): weights, inputs, outputs, the reference criterions' loss terms, gradients, its
+  SequenceGenerator's token ids, its compute_mask_indices draws, its encoder / extractor / synthesis outputs at real
+  width and length, its meters, arch presets, criterion defaults and option tables. The oracle and the plugin are
+  compared with them to fp32 round-off (tolerances in each test). These run everywhere (no reference tree needed).
+* where the reference tree is available, the fixtures are also regenerated in memory and must be identical to the
+  committed ones (stale-fixture guard).
 """
 import os
 import sys
@@ -22,7 +22,7 @@ sys.path.insert(0, GOLD)
 import make_golden_from_ref as mg  # noqa: E402  (constants + case builders; touches the reference only inside cases)
 from oracle import ref_loader as rl  # noqa: E402
 
-needs_ref = pytest.mark.skipif(not rl.available(), reason="reference tree not mounted (GPU box): fixtures only")
+needs_ref = pytest.mark.skipif(not rl.available(), reason="reference tree not available: the stale-fixture guard regenerates from it")
 FP32 = 2e-5   # relative L2, fp32 forward of a 2+2-layer model: different summation orders only
 GRAD = 2e-4   # relative L2 of fp32 gradients
 
@@ -214,96 +214,193 @@ def test_committed_fixture_is_what_the_reference_produces_now(name):
             np.testing.assert_allclose(a, b, rtol=1e-5, atol=1e-6, err_msg=k)
 
 
-@needs_ref
-@pytest.mark.parametrize("T", [199, 499])
-def test_reference_encoder_at_asr_lengths_matches_oracle(T):
-    """VERDICT r1 item 2: `TransformerEncoder.forward` of the reference at T = 199 / 499 (relative positions clipped at
-    +-160, key padding) against the oracle encoder, Base width, 2 layers."""
-    from argparse import Namespace
-    from oracle.speecht5_oracle import TransformerEncoder, base_args
-    ns = rl.load()
-    over = dict(encoder_layers=2, dropout=0.0, attention_dropout=0.0, activation_dropout=0.0, encoder_layerdrop=0.0)
-    rargs = rl.reference_args(**over)
-    torch.manual_seed(3)
-    enc_ref = ns.encoder.TransformerEncoder(rargs, rl.RefDictionary(mg.VOCAB), None).eval()
-    oargs = base_args(**over)
-    enc = TransformerEncoder(oargs, mg.VOCAB, None).eval()
-    enc.load_state_dict(enc_ref.state_dict())
+# ------------------------------------------------------------------ reference observations (tests/golden/ref_pins.npz)
+# What the reference's own modules / functions return, written by tests/golden/make_golden_ref_pins.py. Weights are not
+# stored: both sides fill their parameters from the parameter NAME (seed_parameters), so the same names get the same values.
+def seeded_tensors(shapes, seed):
+    """name -> tensor of that shape, drawn from a generator seeded by the name: scalars and norm weights near 1, biases
+    near 0, other weights ~ N(0, 1 / fan_in)."""
+    import zlib
+    out = {}
+    for name, shape in shapes.items():
+        g = torch.Generator().manual_seed((zlib.crc32(name.encode()) + seed) % (2 ** 31))
+        t = torch.randn(tuple(shape), generator=g)
+        if len(shape) == 0:  # scalar scales (positional-encoding alpha)
+            t = 1.0 + 0.05 * t
+        elif len(shape) == 1:
+            t = 1.0 + 0.05 * t if name.endswith("weight") else 0.02 * t
+        else:
+            t = t * (t[0].numel() ** -0.5)
+        out[name] = t
+    return out
+
+
+def seed_parameters(module, seed):
+    vals = seeded_tensors({n: tuple(p.shape) for n, p in module.named_parameters()}, seed)
+    with torch.no_grad():
+        for n, p in module.named_parameters():
+            p.copy_(vals[n])
+
+
+def output_sample(t, n=8192):
+    """A fixed seeded sample of a tensor's elements (float64)."""
+    flat = t.detach().reshape(-1).double()
+    idx = torch.randint(0, flat.numel(), (n,), generator=torch.Generator().manual_seed(0))
+    return flat[idx]
+
+
+ENC_OVER = dict(encoder_layers=2, dropout=0.0, attention_dropout=0.0, activation_dropout=0.0, encoder_layerdrop=0.0)
+
+
+def encoder_input(T):
     x = torch.randn(2, T, 768, generator=torch.Generator().manual_seed(1))
     pad = torch.zeros(2, T, dtype=torch.bool)
     pad[1, T - 37:] = True
+    return x, pad
+
+
+def conv_extractor_input():
+    return torch.randn(2, 16000, generator=torch.Generator().manual_seed(1)) * 0.1
+
+
+GEN_OVER = dict(mg.TINY, conv_feature_layers=mg.TINY_CONV, conv_pos=16, conv_pos_groups=4)
+
+
+def generate_speech_inputs():
+    g = torch.Generator().manual_seed(2)
+    toks = torch.randint(4, 70, (1, 12), generator=g)
+    spk = torch.randn(1, 512, generator=g)
+    return toks, spk
+
+
+REDUCE_LOGS = [
+    {"t2s": {"loss": 1.5, "l1_loss": 1.0, "l2_loss": 2.0, "bce_loss": 0.5, "sample_size": 1, "ntokens": 100, "nsentences": 4,
+             "enc_dec_attn_loss": 0.01, "encoder_alpha": 1.0, "decoder_alpha": 1.1}, "sample_size": 1, "loss": 1.5},
+    {"t2s": {"loss": 2.5, "l1_loss": 1.0, "l2_loss": 2.0, "bce_loss": 0.5, "sample_size": 1, "ntokens": 100, "nsentences": 4,
+             "enc_dec_attn_loss": 0.01, "encoder_alpha": 1.0, "decoder_alpha": 1.1}, "sample_size": 1, "loss": 2.5},
+    {"s2t": {"loss": 80.0, "ce_loss": 60.0, "ctc_loss": 100.0, "nll_loss": 55.0, "ntokens": 37, "nsentences": 3,
+             "sample_size": 3, "n_correct": 11, "total": 37, "c_errors": 5, "c_total": 30, "w_errors": 2, "wv_errors": 3,
+             "w_total": 9}, "sample_size": 1, "loss": 80.0 / 3},
+    {"text_pretrain": {"loss": 12.0, "bart_loss": 12.0, "ntokens": 50, "sample_size": 50, "loss_prob_perplexity": 0.3,
+                       "code_perplexity": 17.0}, "sample_size": 1, "loss": 0.24},
+    {"speech_pretrain": {"loss": 9.0, "ntokens": 20, "sample_size": 20, "dec_loss": 1.0, "l1_loss": 0.5, "l2_loss": 0.6,
+                         "bce_loss": 0.1, "ngpu": 1, "count_m_0": 12, "correct_m_0": 5, "loss_m_0": 7.0,
+                         "enc_dec_attn_loss": 0.02}, "sample_size": 1, "loss": 0.45},
+]
+ARCHS = ["t5_transformer", "t5_transformer_base", "t5_transformer_large", "t5_transformer_base_asr"]
+
+
+def jsonable(x):
+    """The value as it reads back from the golden file's JSON (tuples -> lists, callables / objects -> their names)."""
+    import json
+    return json.loads(json.dumps(x, default=lambda v: getattr(v, "__name__", repr(v))))
+
+
+def dataclass_defaults(cls):
+    import dataclasses
+    out = {}
+    for f in dataclasses.fields(cls):
+        if f.default is not dataclasses.MISSING:
+            out[f.name] = f.default
+        elif f.default_factory is not dataclasses.MISSING:
+            out[f.name] = f.default_factory()
+    return out
+
+
+def add_args_table(cls):
+    import argparse
+    p = argparse.ArgumentParser(allow_abbrev=False)
+    cls.add_args(p)
+    return p, {a.dest: (tuple(a.option_strings), type(a).__name__, getattr(a.type, "__name__", a.type),
+                        tuple(a.choices) if a.choices else None) for a in p._actions if a.dest != "help"}
+
+
+def task_add_argument_calls(src):
+    """flag -> keyword arguments of every add_argument call in a source text (help / metavar dropped)."""
+    import ast
+    ref = {}
+    for node in ast.walk(ast.parse(src)):
+        if isinstance(node, ast.Call) and isinstance(node.func, ast.Attribute) and node.func.attr == "add_argument":
+            flags = [a.value for a in node.args if isinstance(a, ast.Constant)]
+            kw = {}
+            for k in node.keywords:
+                if k.arg in ("help", "metavar"):
+                    continue
+                try:
+                    kw[k.arg] = ast.literal_eval(k.value)
+                except ValueError:
+                    kw[k.arg] = getattr(k.value, "id", None) or ast.unparse(k.value)
+            ref[flags[-1]] = kw
+    return ref
+
+
+def _pins():
+    import json
+    blob = np.load(os.path.join(GOLD, "ref_pins.npz"))
+    return json.loads(str(blob["meta"])), blob
+
+
+@pytest.mark.parametrize("T", [199, 499])
+def test_reference_encoder_at_asr_lengths_matches_oracle(T):
+    """`TransformerEncoder.forward` of the reference at T = 199 / 499 (relative positions clipped at +-160, key padding)
+    against the oracle encoder, Base width, 2 layers, same parameters by name."""
+    from oracle.speecht5_oracle import TransformerEncoder, base_args
+    meta, blob = _pins()
+    enc = TransformerEncoder(base_args(**ENC_OVER), mg.VOCAB, None).eval()
+    assert sorted(n for n, _ in enc.named_parameters()) == meta["encoder_params"]
+    seed_parameters(enc, 3)
+    x, pad = encoder_input(T)
     with torch.no_grad():
-        a = enc_ref(x, pad)
         b = enc(x, pad)
-    assert rel(b["encoder_out"][0], a["encoder_out"][0]) < 1e-5
-    assert rel(b["encoder_out_for_ctc"][0], a["encoder_out_for_ctc"][0]) < 1e-5
+    assert rel(output_sample(b["encoder_out"][0]), blob[f"encoder/{T}/out"]) < 1e-5
+    assert rel(output_sample(b["encoder_out_for_ctc"][0]), blob[f"encoder/{T}/ctc"]) < 1e-5
 
 
-@needs_ref
 def test_reference_conv_feature_extractor_real_width_matches_oracle():
     """ConvFeatureExtractionModel (speech_encoder_prenet.py:277-374) at the real 512 channels, both modes, 1 s of audio."""
     from oracle.speecht5_oracle_asr import CONV_FEATURE_LAYERS, ConvFeatureExtractionModel, reference_to_oracle_keys
-    ns = rl.load()
-    x = torch.randn(2, 16000, generator=torch.Generator().manual_seed(1)) * 0.1
+    meta, blob = _pins()
+    x = conv_extractor_input()
     for mode in ("default", "layer_norm"):
-        torch.manual_seed(5)
-        ref = ns.speech_encoder_prenet.ConvFeatureExtractionModel(CONV_FEATURE_LAYERS, 0.0, mode, False).eval()
         orc = ConvFeatureExtractionModel(CONV_FEATURE_LAYERS, mode, False).eval()
-        orc.load_state_dict(reference_to_oracle_keys(ref.state_dict()))
+        sd = orc.state_dict()
+        ref_params = seeded_tensors(meta[f"conv/{mode}/shapes"], 5)  # the reference's parameters, filled by name
+        sd.update(reference_to_oracle_keys(ref_params))
+        orc.load_state_dict(sd)
         with torch.no_grad():
-            assert rel(orc(x), ref(x)) < 1e-5, mode
+            assert rel(output_sample(orc(x)), blob[f"conv/{mode}/out"]) < 1e-5, mode
 
 
-@needs_ref
 def test_reference_generate_speech_matches_oracle_autoregressive_synthesis():
     """`T5TransformerModel.generate_speech` (models/speecht5.py:1188-1249; its always-on prenet dropout disabled with
     dprenet_dropout_rate 0) against the oracle's synthesis loop: same number of frames, same mel."""
     from oracle.speecht5_oracle import T5TransformerModelOracle, base_args
-    over = dict(mg.TINY, conv_feature_layers=mg.TINY_CONV, conv_pos=16, conv_pos_groups=4)
-    torch.manual_seed(21)
-    ref = rl.build_reference_model(rl.reference_args(**over), rl.RefTask(mg.VOCAB, "t2s")).eval()
+    meta, blob = _pins()
     orc = T5TransformerModelOracle(base_args(**mg.TINY)).eval()
-    orc.load_state_dict({k: v for k, v in ref.state_dict().items() if k in orc.state_dict()})
-    g = torch.Generator().manual_seed(2)
-    toks = torch.randint(4, 70, (1, 12), generator=g)
-    spk = torch.randn(1, 512, generator=g)
+    missing = sorted(n for n, _ in orc.named_parameters() if n not in set(meta["generate_params"]))
+    assert missing == [], missing
+    seed_parameters(orc, 21)
+    toks, spk = generate_speech_inputs()
     with torch.no_grad():
-        a = ref.generate_speech(source=None, src_tokens=toks, spkembs=spk, threshold=0.5, minlenratio=0.0, maxlenratio=2.0)
         b = orc.generate_speech(src_tokens=toks, spkembs=spk, threshold=0.5, minlenratio=0.0, maxlenratio=2.0)
-    assert a[0].shape == b[0].shape
-    assert rel(b[0], a[0]) < 1e-4
+    want = torch.from_numpy(blob["generate/mel"])
+    assert tuple(b[0].shape) == tuple(want.shape)
+    assert rel(b[0], want) < 1e-4
 
 
-@needs_ref
 def test_reduce_metrics_logs_the_reference_keys_and_values():
-    """SpeechT5Criterion.reduce_metrics (criterions/speecht5_criterion.py:123-436) run by the reference itself and by the
-    plugin on the same logging outputs: same meter names, same values."""
-    import importlib
-    ns = rl.load()
-    ref_cls = importlib.import_module("speecht5.criterions.speecht5_criterion").SpeechT5Criterion
+    """SpeechT5Criterion.reduce_metrics (criterions/speecht5_criterion.py:123-436): the meter names and values the
+    reference logs for these logging outputs (golden file) are what the plugin logs."""
     from speecht5_b200.criterions import SpeechT5Criterion
     from speecht5_b200.fairseq_shim import metrics as ours
-    t2s = {"loss": 1.5, "l1_loss": 1.0, "l2_loss": 2.0, "bce_loss": 0.5, "sample_size": 1, "ntokens": 100,
-           "nsentences": 4, "enc_dec_attn_loss": 0.01, "encoder_alpha": 1.0, "decoder_alpha": 1.1}
-    s2t = {"loss": 80.0, "ce_loss": 60.0, "ctc_loss": 100.0, "nll_loss": 55.0, "ntokens": 37, "nsentences": 3,
-           "sample_size": 3, "n_correct": 11, "total": 37, "c_errors": 5, "c_total": 30, "w_errors": 2, "wv_errors": 3,
-           "w_total": 9}
-    text = {"loss": 12.0, "bart_loss": 12.0, "ntokens": 50, "sample_size": 50, "loss_prob_perplexity": 0.3,
-            "code_perplexity": 17.0}
-    hub = {"loss": 9.0, "ntokens": 20, "sample_size": 20, "dec_loss": 1.0, "l1_loss": 0.5, "l2_loss": 0.6, "bce_loss": 0.1,
-           "ngpu": 1, "count_m_0": 12, "correct_m_0": 5, "loss_m_0": 7.0, "enc_dec_attn_loss": 0.02}
-    logs = [{"t2s": t2s, "sample_size": 1, "loss": 1.5}, {"t2s": dict(t2s, loss=2.5), "sample_size": 1, "loss": 2.5},
-            {"s2t": s2t, "sample_size": 1, "loss": 80.0 / 3}, {"text_pretrain": text, "sample_size": 1, "loss": 0.24},
-            {"speech_pretrain": hub, "sample_size": 1, "loss": 0.45}]
-    ns.metrics.logged.clear()
-    ns.metrics.derived.clear()
-    ref_cls.reduce_metrics(logs)
+    meta, _ = _pins()
     ours.reset()
-    SpeechT5Criterion.reduce_metrics(logs)
-    assert set(ours.scalars) == set(ns.metrics.logged), set(ours.scalars) ^ set(ns.metrics.logged)
-    for k, v in ns.metrics.logged.items():
+    SpeechT5Criterion.reduce_metrics(REDUCE_LOGS)
+    logged = meta["reduce_metrics"]["logged"]
+    assert set(ours.scalars) == set(logged), set(ours.scalars) ^ set(logged)
+    for k, v in logged.items():
         assert abs(float(ours.scalars[k]) - float(v)) < 1e-9, k
-    assert set(ours.derived) == set(ns.metrics.derived)
+    assert set(ours.derived) == set(meta["reduce_metrics"]["derived"])
 
 
 def test_train_step_returns_the_reference_logging_shape():
@@ -373,65 +470,85 @@ def _close(a, b, tol=1e-5):
     return abs(a - b) <= tol * max(1.0, abs(b))
 
 
-@pytest.mark.parametrize("dec_weight,nomask,weights", [(1.0, 0.0, [10.0]), (0.0, 0.5, [10.0, 0.1]), (0.5, 1.0, [10.0, 0.1, 3.0]),
-                                                       (1.0, 0.0, None)])
-def test_speech_pretrain_criterion_equals_the_reference_criterion(dec_weight, nomask, weights):
-    """speecht5_b200/criterions/speech_pretrain_criterion.py against the reference's own SpeechPretrainCriterion
-    (speech_pretrain_criterion.py:50-190, loaded unmodified): loss, sample size, every logging key and the gradients on
-    the model outputs, with / without the decoder branch, the unmasked term and 1 / 2 / 3 configured extra weights."""
-    import importlib
-    from speecht5_b200.criterions import SpeechPretrainCriterion
-    rl.load()
-    ref_mod = importlib.import_module("speecht5.criterions.speech_pretrain_criterion")
-    task = rl.RefTask(mg.VOCAB, "pretrain")
-    kw = dict(pred_masked_weight=1.0, pred_nomask_weight=nomask, loss_weights=None if weights is None else list(weights),
-              log_keys=["temp"], hubert_weight=0.7, dec_weight=dec_weight)
-    ref_crit = ref_mod.SpeechPretrainCriterion(task, True, **kw)
-    kw["loss_weights"] = None if weights is None else list(weights)
-    our_crit = SpeechPretrainCriterion(task, True, **kw)
-    ms_ref, ms_our = _PretrainStub(4), _PretrainStub(4)
-    want, n_want, log_want = ref_crit(ms_ref, _speech_pretrain_sample())
-    got, n_got, log_got = our_crit(ms_our, _speech_pretrain_sample())
-    assert n_got == n_want and _close(got, want)
-    assert set(log_got) == set(log_want), (sorted(log_got), sorted(log_want))
-    for k in log_want:
-        assert _close(log_got[k], log_want[k]), (k, log_got[k], log_want[k])
-    assert ms_our.calls[0].get("only_hubert", False) == ms_ref.calls[0].get("only_hubert", False) == (dec_weight == 0)
-    want.backward()
-    got.backward()
-    for (n, p), q in zip(ms_ref.named_parameters(), ms_our.parameters()):
-        if p.grad is None:
-            assert q.grad is None, n
-        else:
-            assert torch.allclose(q.grad, p.grad, rtol=1e-5, atol=1e-7), n
+# What the reference's own criteria / Dictionary return on these inputs: tests/golden/ref_criteria_dict.npz, written by
+# tests/golden/make_golden_ref_criteria.py (which runs the reference classes unmodified through oracle/ref_loader.py).
+SPEECH_CASES = [(1.0, 0.0, [10.0]), (0.0, 0.5, [10.0, 0.1]), (0.5, 1.0, [10.0, 0.1, 3.0]), (1.0, 0.0, None)]
+TEXT_CASES = [(False, [0.1]), (True, [0.1]), (False, [0.1, 2.0])]
 
 
-@pytest.mark.parametrize("sentence_avg,weights", [(False, [0.1]), (True, [0.1]), (False, [0.1, 2.0])])
-def test_text_pretrain_criterion_equals_the_reference_criterion(sentence_avg, weights):
-    """speecht5_b200/criterions/text_pretrain_criterion.py against the reference's TextPretrainCriterion
-    (text_pretrain_criterion.py:36-105): padded targets, both sample-size modes, and the reference's weight-list rule
-    when more weights than extra terms are configured (it keeps the tail, :74-75)."""
-    import importlib
-    from speecht5_b200.criterions import TextPretrainCriterion
-    rl.load()
-    ref_mod = importlib.import_module("speecht5.criterions.text_pretrain_criterion")
-    task = rl.RefTask(mg.VOCAB, "pretrain")
+def speech_case_key(dec_weight, nomask, weights):
+    return f"dec{dec_weight}_nomask{nomask}_w{weights}"
+
+
+def text_case_key(sentence_avg, weights):
+    return f"avg{sentence_avg}_w{weights}"
+
+
+def _ref_criteria_gold():
+    import json
+    blob = np.load(os.path.join(GOLD, "ref_criteria_dict.npz"))
+    return json.loads(str(blob["meta"])), blob
+
+
+def _text_pretrain_sample(task):
     pad = task.target_dictionary.pad()
     tgt = torch.randint(4, 37, (3, 9), generator=torch.Generator().manual_seed(2))
     tgt[1, 6:] = pad
     tgt[2, 3:] = pad
-    sample = {"net_input": {"src_tokens": None}, "target": tgt, "ntokens": int(tgt.ne(pad).sum()), "task_name": "text_pretrain"}
-    ms_ref, ms_our = _PretrainStub(6, text=True), _PretrainStub(6, text=True)
-    want, n_want, log_want = ref_mod.TextPretrainCriterion(task, sentence_avg, 0.9, list(weights))(ms_ref, sample)
-    got, n_got, log_got = TextPretrainCriterion(task, sentence_avg, 0.9, list(weights))(ms_our, sample)
-    assert n_got == n_want and _close(got, want)
-    assert set(log_got) == set(log_want), (sorted(log_got), sorted(log_want))
-    for k in log_want:
-        assert _close(log_got[k], log_want[k]), (k, log_got[k], log_want[k])
-    want.backward()
+    return {"net_input": {"src_tokens": None}, "target": tgt, "ntokens": int(tgt.ne(pad).sum()), "task_name": "text_pretrain"}
+
+
+@pytest.mark.parametrize("dec_weight,nomask,weights", SPEECH_CASES)
+def test_speech_pretrain_criterion_equals_the_reference_criterion(dec_weight, nomask, weights):
+    """speecht5_b200/criterions/speech_pretrain_criterion.py against the reference's own SpeechPretrainCriterion
+    (speech_pretrain_criterion.py:50-190, run unmodified into the golden file): loss, sample size, every logging key and
+    the gradients on the model outputs, with / without the decoder branch, the unmasked term and 1 / 2 / 3 configured
+    extra weights."""
+    from speecht5_b200.criterions import SpeechPretrainCriterion
+    meta, blob = _ref_criteria_gold()
+    key = speech_case_key(dec_weight, nomask, weights)
+    ref = meta["speech"][key]
+    task = rl.RefTask(mg.VOCAB, "pretrain")
+    kw = dict(pred_masked_weight=1.0, pred_nomask_weight=nomask, loss_weights=None if weights is None else list(weights),
+              log_keys=["temp"], hubert_weight=0.7, dec_weight=dec_weight)
+    our_crit = SpeechPretrainCriterion(task, True, **kw)
+    ms_our = _PretrainStub(4)
+    got, n_got, log_got = our_crit(ms_our, _speech_pretrain_sample())
+    assert n_got == ref["n"] and _close(got, ref["loss"])
+    assert set(log_got) == set(ref["log"]), (sorted(log_got), sorted(ref["log"]))
+    for k, v in ref["log"].items():
+        assert _close(log_got[k], v), (k, log_got[k], v)
+    assert ms_our.calls[0].get("only_hubert", False) == ref["only_hubert"] == (dec_weight == 0)
     got.backward()
-    assert torch.allclose(ms_our.logits.grad, ms_ref.logits.grad, rtol=1e-5, atol=1e-7)
-    assert (ms_ref.pp.grad is None and ms_our.pp.grad is None) or torch.allclose(ms_our.pp.grad, ms_ref.pp.grad)
+    for n, q in ms_our.named_parameters():
+        if n not in ref["grads"]:
+            assert q.grad is None, n
+        else:
+            assert torch.allclose(q.grad, torch.from_numpy(blob[f"speech/{key}/{n}"]), rtol=1e-5, atol=1e-7), n
+
+
+@pytest.mark.parametrize("sentence_avg,weights", TEXT_CASES)
+def test_text_pretrain_criterion_equals_the_reference_criterion(sentence_avg, weights):
+    """speecht5_b200/criterions/text_pretrain_criterion.py against the reference's TextPretrainCriterion
+    (text_pretrain_criterion.py:36-105, run unmodified into the golden file): padded targets, both sample-size modes, and
+    the reference's weight-list rule when more weights than extra terms are configured (it keeps the tail, :74-75)."""
+    from speecht5_b200.criterions import TextPretrainCriterion
+    meta, blob = _ref_criteria_gold()
+    key = text_case_key(sentence_avg, weights)
+    ref = meta["text"][key]
+    task = rl.RefTask(mg.VOCAB, "pretrain")
+    ms_our = _PretrainStub(6, text=True)
+    got, n_got, log_got = TextPretrainCriterion(task, sentence_avg, 0.9, list(weights))(ms_our, _text_pretrain_sample(task))
+    assert n_got == ref["n"] and _close(got, ref["loss"])
+    assert set(log_got) == set(ref["log"]), (sorted(log_got), sorted(ref["log"]))
+    for k, v in ref["log"].items():
+        assert _close(log_got[k], v), (k, log_got[k], v)
+    got.backward()
+    assert torch.allclose(ms_our.logits.grad, torch.from_numpy(blob[f"text/{key}/logits"]), rtol=1e-5, atol=1e-7)
+    if ref["pp_grad"] is None:
+        assert ms_our.pp.grad is None
+    else:
+        assert _close(ms_our.pp.grad, ref["pp_grad"])
 
 
 def _reference_dictionary_class():
@@ -464,27 +581,41 @@ def _reference_dictionary_class():
                 sys.modules[n] = m
 
 
+DICT_WORDS = ["▁", "e", "t", "a", "o", "n", "'", "<weird token>", "zz"]
+DICT_IDS = [[0, 5, 6, 3, 2, 1], [7, 8, 4, 2, 1, 1]]
+
+
+def dict_file_text():
+    return "".join(f"{w} {100 - i}\n" for i, w in enumerate(DICT_WORDS))
+
+
+def dictionary_observations(d):
+    """Everything the test compares, from a loaded `dict.txt` (DICT_WORDS): the same calls on either implementation."""
+    ids = torch.tensor(DICT_IDS)
+    obs = {"len": len(d), "symbols": list(d.symbols), "indices": dict(d.indices),
+           "specials": [d.bos(), d.pad(), d.eos(), d.unk()], "index": [d.index(w) for w in DICT_WORDS + ["missing", "<pad>"]]}
+    obs["add"] = [d.add_symbol("<mask>"), d.add_symbol("e")]
+    obs["count"] = list(d.count)
+    obs["item999"] = d[999]
+    obs["string"] = [d.string(ids, extra_symbols_to_ignore={1}), d.string(ids[0], include_eos=True, unk_string="?")]
+    return obs
+
+
 def test_vocabulary_files_load_like_the_reference_dictionary(tmp_path):
     """speecht5_b200/dictionary.py (what SpeechT5Task.setup_task loads `dict.txt` / `dict.<label>.txt` with when fairseq
-    is not importable) against the reference's own fairseq Dictionary: same indices, length, lookups, appended task
-    symbols and id -> text conversion; then the task built from a data directory (tasks/speecht5.py:272-318)."""
+    is not importable) against the reference's own fairseq Dictionary (its observations in the golden file): same
+    indices, length, lookups, appended task symbols and id -> text conversion; then the task built from a data directory
+    (tasks/speecht5.py:272-318)."""
     from speecht5_b200.dictionary import Vocabulary
     from speecht5_b200.tasks import SpeechT5Task
     from speecht5_b200.models import make_args
-    Ref = _reference_dictionary_class()
-    words = ["▁", "e", "t", "a", "o", "n", "'", "<weird token>", "zz"]
-    (tmp_path / "dict.txt").write_text("".join(f"{w} {100 - i}\n" for i, w in enumerate(words)), encoding="utf-8")
+    meta, _ = _ref_criteria_gold()
+    words = DICT_WORDS
+    (tmp_path / "dict.txt").write_text(dict_file_text(), encoding="utf-8")
     (tmp_path / "dict.km.txt").write_text("".join(f"{i} 1\n" for i in range(25)), encoding="utf-8")
-    ref, got = Ref.load(str(tmp_path / "dict.txt")), Vocabulary.load(str(tmp_path / "dict.txt"))
-    assert len(got) == len(ref) == 4 + len(words) and got.symbols == ref.symbols and got.indices == ref.indices
-    assert (got.bos(), got.pad(), got.eos(), got.unk()) == (ref.bos(), ref.pad(), ref.eos(), ref.unk()) == (0, 1, 2, 3)
-    for w in words + ["missing", "<pad>"]:
-        assert got.index(w) == ref.index(w)
-    assert got.add_symbol("<mask>") == ref.add_symbol("<mask>") and got.add_symbol("e") == ref.add_symbol("e")
-    assert got.count == ref.count and got[999] == ref[999]
-    ids = torch.tensor([[0, 5, 6, 3, 2, 1], [7, 8, 4, 2, 1, 1]])
-    assert got.string(ids, extra_symbols_to_ignore={1}) == ref.string(ids, extra_symbols_to_ignore={1})
-    assert got.string(ids[0], include_eos=True, unk_string="?") == ref.string(ids[0], include_eos=True, unk_string="?")
+    got = dictionary_observations(Vocabulary.load(str(tmp_path / "dict.txt")))
+    assert got == meta["dictionary"]
+    assert got["len"] == 4 + len(words) and got["specials"] == [0, 1, 2, 3]
     (tmp_path / "dup.txt").write_text("a 1\na 2\n")
     with pytest.raises(RuntimeError):
         Vocabulary.load(str(tmp_path / "dup.txt"))
@@ -501,70 +632,47 @@ def test_vocabulary_files_load_like_the_reference_dictionary(tmp_path):
     assert model.hubert_layer is not None
 
 
-@needs_ref
-@pytest.mark.parametrize("arch", ["t5_transformer", "t5_transformer_base", "t5_transformer_large", "t5_transformer_base_asr"])
+@pytest.mark.parametrize("arch", ARCHS)
 def test_arch_presets_equal_the_reference_arch_functions(arch):
     """models/speecht5.py:1252-1447: every option both sides know gets the value the reference's OWN arch function
-    assigns (run unmodified through oracle/ref_loader.py) -- layer counts, widths, dropouts, extractor mode, final_dim,
-    codebook sizes, positional options: what decides whether a reference checkpoint loads and trains the same."""
+    assigns (stored in the golden file) -- layer counts, widths, dropouts, extractor mode, final_dim, codebook sizes,
+    positional options: what decides whether a reference checkpoint loads and trains the same."""
     from speecht5_b200.models import make_args
-    ref = vars(rl.reference_args(arch=arch))
-    ours = vars(make_args(arch))
+    meta, _ = _pins()
+    ref = meta["arch"][arch]
+    ours = jsonable(vars(make_args(arch)))
     shared = [k for k in ours if k in ref]
     assert len(shared) >= 80
     for k in ("final_dim", "latent_vars", "latent_groups", "latent_temp", "codebook_prob", "logit_temp", "extractor_mode",
               "use_conv_pos", "use_sinc_pos", "untie_final_proj", "label_rates"):
         assert k in shared, k
-    def same(a, b):
-        return tuple(a) == tuple(b) if isinstance(a, (list, tuple)) and isinstance(b, (list, tuple)) else a == b
-    diff = {k: (ours[k], ref[k]) for k in shared if not same(ours[k], ref[k])}
+    diff = {k: (ours[k], ref[k]) for k in shared if ours[k] != ref[k]}
     assert not diff, diff
 
 
-@needs_ref
 def test_criterion_config_defaults_equal_the_reference_dataclass():
     """speecht5_criterion.py:23-30: fairseq builds the criterion from this dataclass, so its defaults decide what a
-    recipe that omits a flag trains with. Every field both sides define has the reference's default (sentence_avg is an
-    interpolation of optimization.sentence_avg there)."""
-    import dataclasses
-    import importlib
+    recipe that omits a flag trains with. Every field both sides define has the reference's default (stored in the
+    golden file; sentence_avg is an interpolation of optimization.sentence_avg there)."""
     from speecht5_b200.criterions.speecht5_criterion import SpeechT5CriterionConfig
-    rl.load()
-    ref_cls = importlib.import_module("speecht5.criterions.speecht5_criterion").SpeechT5CriterionConfig
-
-    def defaults(cls):
-        out = {}
-        for f in dataclasses.fields(cls):
-            if f.default is not dataclasses.MISSING:
-                out[f.name] = f.default
-            elif f.default_factory is not dataclasses.MISSING:
-                out[f.name] = f.default_factory()
-        return out
-    ref, ours = defaults(ref_cls), defaults(SpeechT5CriterionConfig)
+    meta, _ = _pins()
+    ref, ours = meta["criterion_defaults"], jsonable(dataclass_defaults(SpeechT5CriterionConfig))
     shared = [k for k in ours if k in ref and k != "sentence_avg"]
     assert len(shared) >= 20
-    diff = {k: (ours[k], ref[k]) for k in shared
-            if (list(ours[k]) != list(ref[k]) if isinstance(ours[k], (list, tuple)) else ours[k] != ref[k])}
+    diff = {k: (ours[k], ref[k]) for k in shared if ours[k] != ref[k]}
     assert not diff, diff
 
 
-@needs_ref
 def test_model_command_line_options_cover_the_reference_add_args():
-    """models/speecht5.py:117-560 (T5TransformerModel.add_args of the reference, run unmodified): every option it
-    defines is defined here with the same value type and choices, so a recipe's command line -- README fine-tuning
-    commands pass --freeze-encoder-updates, --mask-prob, --mask-channel-prob, --feature-grad-mult -- parses under this
-    plugin; ours adds only the two opt-in builders."""
-    import argparse
+    """models/speecht5.py:117-560 (T5TransformerModel.add_args of the reference; its option table is in the golden
+    file): every option it defines is defined here with the same value type and choices, so a recipe's command line --
+    README fine-tuning commands pass --freeze-encoder-updates, --mask-prob, --mask-channel-prob, --feature-grad-mult --
+    parses under this plugin; ours adds only the two opt-in builders."""
     from speecht5_b200.models import T5TransformerModel
-    ns = rl.load()
-
-    def opts(cls):
-        p = argparse.ArgumentParser(allow_abbrev=False)
-        cls.add_args(p)
-        return p, {a.dest: (tuple(a.option_strings), type(a).__name__, getattr(a.type, "__name__", a.type),
-                            tuple(a.choices) if a.choices else None) for a in p._actions if a.dest != "help"}
-    _, ref = opts(ns.T5TransformerModel)
-    parser, ours = opts(T5TransformerModel)
+    meta, _ = _pins()
+    ref = meta["model_add_args"]
+    parser, ours = add_args_table(T5TransformerModel)
+    ours = jsonable(ours)
     assert sorted(k for k in ref if k not in ours) == []
     assert sorted(k for k in ours if k not in ref) == ["build_speech_encoder", "build_text_decoder"]
     loose = {"latent_temp", "mask_selection", "mask_channel_selection"}  # (str vs literal_eval / untyped: same strings accepted)
@@ -577,33 +685,21 @@ def test_model_command_line_options_cover_the_reference_add_args():
     assert not hasattr(got, "encoder_layers")  # unset options fall through to the arch function
 
 
-@needs_ref
 def test_task_command_line_options_equal_the_reference_add_args():
-    """tasks/speecht5.py:44-213 (SpeechT5Task.add_args; the module itself needs fairseq's data package, so its
-    add_argument calls are read from the source text): same flags, value types, defaults, choices and actions here."""
-    import ast
+    """tasks/speecht5.py:44-213 (SpeechT5Task.add_args; the module itself needs fairseq's data package, so the generator
+    reads its add_argument calls from the source text into the golden file): same flags, value types, defaults, choices
+    and actions here."""
     from speecht5_b200.tasks.speecht5 import SpeechT5Task
-    src = open("/root/reference/SpeechT5/speecht5/tasks/speecht5.py").read()
-    ref = {}
-    for node in ast.walk(ast.parse(src)):
-        if isinstance(node, ast.Call) and isinstance(node.func, ast.Attribute) and node.func.attr == "add_argument":
-            flags = [a.value for a in node.args if isinstance(a, ast.Constant)]
-            kw = {}
-            for k in node.keywords:
-                if k.arg in ("help", "metavar"):
-                    continue
-                try:
-                    kw[k.arg] = ast.literal_eval(k.value)
-                except ValueError:
-                    kw[k.arg] = getattr(k.value, "id", None) or ast.unparse(k.value)
-            ref[flags[-1]] = kw
+    meta, _ = _pins()
+    ref = meta["task_add_args"]
     ours = {}
     for flag, kw in SpeechT5Task._OPTIONS:
         kw = {k: (getattr(v, "__name__", v) if k == "type" else v) for k, v in kw.items() if k not in ("help", "metavar")}
         ours[flag] = kw
+    ours = jsonable(ours)
     assert sorted(k for k in ref if k not in ours) == ["data"]  # (the positional argument, added in add_args itself)
     assert sorted(k for k in ours if k not in ref) == []
-    ref["--t5-task"]["choices"] = SpeechT5Task.TASK_NAME  # (the reference names its list the same way, :40)
+    ref["--t5-task"]["choices"] = jsonable(SpeechT5Task.TASK_NAME)  # (the reference names its list the same way, :40)
     diff = {k: (ours[k], ref[k]) for k in ours if ours[k] != ref[k]}
     assert not diff, diff
     assert len(ours) >= 35

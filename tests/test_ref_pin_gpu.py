@@ -104,8 +104,8 @@ def test_tts_forward_loss_gradients_against_reference_vectors(cuda, name, pre_ln
     else:
         # throughput mode on a 2 + 2 layer, 64-wide model whose attention the fixture sharpens (q, k x6): single small
         # gradients (the first post-net conv behind BatchNorm over 2 utterances, k_proj of a peaked softmax) carry
-        # 0.15-0.45 of bf16 noise on EVERY attention path, the exact fp32 row kernels included (tools/diag_grad_bf16.py,
-        # profiles/r02_diag_grad_bf16.txt). Bound the worst one (cosine > 0.8) and the typical one.
+        # 0.15-0.45 of bf16 noise on EVERY attention path, the exact fp32 row kernels included. Bound the worst one
+        # (cosine > 0.8) and the typical one.
         vals = sorted(errs.values())
         assert vals[-1] < 0.6, max(errs.items(), key=lambda kv: kv[1])
         assert vals[len(vals) // 2] < 0.25, errs

@@ -74,7 +74,7 @@ def test_two_rank_exchange_equals_two_micro_batches_on_one_rank(mode):
     """legacy_distributed_data_parallel.py:76-165 + trainer.py:776-826: the mean over ranks of per-rank normalised
     gradients. Both exchanges (reduce-scatter + sharded Adam + all-gather; per-stage all-reduce) give the parameters a
     single process reaches with the two batches as micro-batches; every stage's exchange is launched from its backward
-    hook (ADVICE r1: the old hook never fired)."""
+    hook."""
     ref, tr1 = _run_single(torch.bfloat16)
     gn1 = tr1.grad_norm()
     ctx = mp.get_context("spawn")
@@ -131,7 +131,7 @@ def test_optimizer_state_round_trip_and_overflow_guard():
 
 
 def test_static_shadows_follow_load_state_dict():
-    """ADVICE r1: fairseq builds the trainer first and loads the checkpoint second; the flat bf16 shadow the GEMMs read
+    """fairseq builds the trainer first and loads the checkpoint second; the flat bf16 shadow the GEMMs read
     must follow."""
     from speecht5_b200.ops import RT
     from speecht5_b200.trainer import B200Trainer

@@ -1,7 +1,7 @@
-"""Round-2 measurement of the inference-side rows (SURVEY 8a rows 15, 16, 21) on one B200, CUDA-event timed after a
+"""Measurement of the inference-side rows (SURVEY 8a rows 15, 16, 21) on one GPU, CUDA-event timed after a
 warm-up: greedy synthesis with prefix recomputation vs the key/value cache (fixed number of decoder steps), the HiFi-GAN
 generator and the log-mel front end, each with the CPU oracle timed next to it on a small sample.
-usage (GPU box): python tools/bench_inference.py [--steps 100] > gpurun_out/bench_inference.json"""
+usage: python tools/bench_inference.py [--steps 100] > bench_inference.json"""
 import argparse
 import json
 import os

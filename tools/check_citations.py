@@ -8,7 +8,7 @@ import re
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("ST5_REFERENCE_ROOT", "/root/reference")  # the same root as oracle/ref_loader.py
 ALIAS = {"legacy_ddp.py": "fairseq/distributed/legacy_distributed_data_parallel.py"}  # SURVEY.md:15 shorthand
 PAT = re.compile(r"([A-Za-z0-9_./-]+\.py):(\d+)(?:-(\d+))?")
 
