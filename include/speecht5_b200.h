@@ -55,7 +55,7 @@ int st5_device_ok(void);
  * epi(v) = dropout(act(v + c_old*accumulate + bias[n] + bias2[m / bias2_rows][n])) + residual[m][n]; the value before
  * act() is also stored to c_pre when non-null.
  * accumulate: 0 = overwrite; 1 = c += (read-modify-write in the epilogue, FP32 c); 2 = c += as a TMA reduce-add at the
- * L2 (FP32 c, 16-byte aligned rows): batch entries may then SHARE one output (c_bs = 0) -- a contraction split over the
+ * L2 (FP32 c, 16-byte aligned rows, N a multiple of 4): batch entries may then SHARE one output (c_bs = 0) -- a contraction split over the
  * batch dimension (weight gradients: a_bs / b_bs step along K) -- and nothing reads c first. */
 typedef struct st5_gemm_args {
   int32_t M, N, K, nb1, nb2;

@@ -602,14 +602,17 @@ static int launch_variant(const GemmDesc& g, const EpiParams& ep, cudaStream_t s
   if (total > 0x7fffffffL) return -4;
   e2.num_tiles = (int)total;
   // Output maps for the TMA-store epilogue: 32x32 element boxes, 64B (bf16) / 128B (fp32) swizzle. Needs 16-byte
-  // aligned bases and row / batch pitches; otherwise the epilogue falls back to per-thread stores.
+  // aligned bases and row / batch pitches, and a row length of whole 16-byte units: the bulk store clips a box at the
+  // edge of the tensor in 16-byte units, so with a ragged N it also writes the columns [N, c_ld) up to the next 16-byte
+  // boundary (zeros, over whatever the caller keeps there). Otherwise the epilogue falls back to per-thread stores.
   CUtensorMap mc, mcp;
   memset(&mc, 0, sizeof(mc));
   memset(&mcp, 0, sizeof(mcp));
   e2.tma_store = 0;
   {
     const long es = g.c_fp32 ? 4 : 2;
-    const bool ok = ((g.c_ld * es) % 16 == 0) && (g.nb1 <= 1 || (g.c_bs1 * es) % 16 == 0) &&
+    const bool ok = (((long)g.N * es) % 16 == 0) && ((g.c_ld * es) % 16 == 0) &&
+                    (g.nb1 <= 1 || (g.c_bs1 * es) % 16 == 0) &&
                     (g.nb2 <= 1 || (g.c_bs2 * es) % 16 == 0) && (reinterpret_cast<uintptr_t>(g.C) % 16 == 0) &&
                     (g.C_pre == nullptr || reinterpret_cast<uintptr_t>(g.C_pre) % 16 == 0);
     if (ok) {

@@ -7,21 +7,52 @@ import math
 import torch
 
 
-def _view(t, nb1, rows, K, mn, ld, bs1):
+def _view(t, nb1, rows, K, mn, ld, bs1, nb2=1, bs2=0):
+    """[nb2 * nb1, rows, K] view of an operand (batch index z = b2 * nb1 + b1; a stride of 0 broadcasts)."""
     base = t.storage_offset()
     if mn:  # memory [K][ld], row index contiguous
-        v = torch.as_strided(t, (nb1, K, rows), (bs1, ld, 1), base)
-        return v.transpose(1, 2)
-    return torch.as_strided(t, (nb1, rows, K), (bs1, ld, 1), base)
+        v = torch.as_strided(t, (nb2, nb1, K, rows), (bs2, bs1, ld, 1), base).transpose(2, 3)
+    else:
+        v = torch.as_strided(t, (nb2, nb1, rows, K), (bs2, bs1, ld, 1), base)
+    return v.reshape(nb2 * nb1, rows, K)
 
 
 def _gelu_grad(z):
     return 0.5 * (1 + torch.erf(z / math.sqrt(2))) + z * torch.exp(-0.5 * z * z) / math.sqrt(2 * math.pi)
 
 
+def _tanh_u(z):
+    return torch.tanh(math.sqrt(2 / math.pi) * (z + 0.044715 * z ** 3))
+
+
+def _gelu_tanh(z):
+    """The tanh form of GELU the kernels evaluate for act = gelu_tanh (include/speecht5_b200.h ST5_ACT_GELU_TANH)."""
+    return 0.5 * z * (1 + _tanh_u(z))
+
+
+def _gelu_tanh_grad(z):
+    t = _tanh_u(z)
+    return 0.5 * (1 + t) + 0.5 * z * (1 - t * t) * math.sqrt(2 / math.pi) * (1 + 3 * 0.044715 * z * z)
+
+
+def _act(v, act):
+    if act == "gelu":
+        return torch.nn.functional.gelu(v)
+    if act in ("gelu_tanh", "gelu_tanh_gate"):
+        return _gelu_tanh(v)
+    if act == "relu":
+        return torch.relu(v)
+    if act == "tanh":
+        return torch.tanh(v)
+    assert act in (None, "none"), act
+    return v
+
+
 def _act_grad(z, act):
-    if act in ("gelu", "gelu_tanh"):
+    if act == "gelu":
         return _gelu_grad(z)
+    if act == "gelu_tanh":
+        return _gelu_tanh_grad(z)
     if act == "relu":
         return (z > 0).to(z.dtype)
     if act == "tanh":
@@ -29,52 +60,76 @@ def _act_grad(z, act):
     raise AssertionError(act)
 
 
+def gemm_keep(M, N, nb, drop_p, seed, offset):
+    """[nb, M, N] keep mask of the GEMM epilogue's dropout: element (z, m, n) has index (z * M + m) * N + n -- the logical
+    output, whatever c_ld and the batch strides are (tests/dropout_ref.py states the generator)."""
+    import numpy as np
+    import dropout_ref
+    idx = (np.arange(nb, dtype=np.uint64)[:, None, None] * np.uint64(M) + np.arange(M, dtype=np.uint64)[:, None]) \
+        * np.uint64(N) + np.arange(N, dtype=np.uint64)
+    return torch.from_numpy(dropout_ref.keep_mask(seed, offset, idx, drop_p))
+
+
 def gemm(a, b, out, *, M, N, K, a_mn=False, b_mn=False, a_ld=None, b_ld=None, c_ld=None, nb1=1, nb2=1, a_bs=(0, 0),
          b_bs=(0, 0), c_bs=(0, 0), bias=None, bias2=None, bias2_rows=0, residual=None, c_pre=None, act=None, alpha=1.0,
          accumulate=False, drop_p=0.0, seed=0, offset=0, actgrad_pre=None, actgrad_act=None):
-    assert nb2 == 1 and drop_p == 0.0
+    """st5_gemm_bf16 in fp64: out[z] = dropout(act(alpha * A[z] B[z]^T + c_old + bias + bias2)) * act'(actgrad_pre)
+    + residual, z = b2 * nb1 + b1; c_pre receives the value before act() (for gelu_tanh_gate: keep * scale *
+    gelu_tanh'(x) instead). bias2 row m is bias2[m // bias2_rows] at a row pitch of N, the same for every batch entry
+    (the kernel does not index it by z)."""
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
+    assert not (int(offset) >> 63), "device-resident seeds: pass the seed value itself"
     a_ld = a_ld if a_ld is not None else (M if a_mn else K)
     b_ld = b_ld if b_ld is not None else (N if b_mn else K)
     c_ld = c_ld if c_ld is not None else N
-    for t, ld, bs in ((a, a_ld, a_bs[0]), (b, b_ld, b_bs[0])):  # what cuTensorMapEncodeTiled demands of an operand
-        assert (t.storage_offset() * 2) % 16 == 0 and (ld * 2) % 16 == 0 and (bs * 2) % 16 == 0, "TMA alignment"
-    A = _view(a, nb1, M, K, a_mn, a_ld, a_bs[0]).double()
-    B = _view(b, nb1, N, K, b_mn, b_ld, b_bs[0]).double()
-    v = alpha * torch.bmm(A, B.transpose(1, 2))
+    for t, ld, bs in ((a, a_ld, a_bs), (b, b_ld, b_bs)):  # what cuTensorMapEncodeTiled demands of an operand
+        assert (t.storage_offset() * 2) % 16 == 0 and (ld * 2) % 16 == 0, "TMA alignment"
+        assert (bs[0] * 2) % 16 == 0 and (bs[1] * 2) % 16 == 0, "TMA alignment"
+    nb = nb1 * nb2
+    A = _view(a, nb1, M, K, a_mn, a_ld, a_bs[0], nb2, a_bs[1]).double()
+    B = _view(b, nb1, N, K, b_mn, b_ld, b_bs[0], nb2, b_bs[1]).double()
+    v = (alpha * torch.bmm(A, B.transpose(1, 2))).reshape(nb2, nb1, M, N)
+
+    def out_view(t):
+        return torch.as_strided(t, (nb2, nb1, M, N), (c_bs[1], c_bs[0], c_ld, 1), t.storage_offset())
+    shared = (nb1 > 1 and c_bs[0] == 0) or (nb2 > 1 and c_bs[1] == 0)
     if int(accumulate) == 2:  # L2-side accumulate: batch entries may share one output (c_bs = 0), split-K
         assert out.dtype == torch.float32 and (c_ld * 4) % 16 == 0 and bias is None and c_pre is None and act in (None, "none")
-        if nb1 > 1 and c_bs[0] == 0:
-            C1 = torch.as_strided(out, (M, N), (c_ld, 1), out.storage_offset())
-            C1.copy_((C1.double() + v.sum(0)).to(out.dtype))
-            return out
-    assert not (nb1 > 1 and c_bs[0] == 0), "several batch entries into one output need accumulate = 2"
-    C = torch.as_strided(out, (nb1, M, N), (c_bs[0], c_ld, 1), out.storage_offset())
+        assert bias2 is None and residual is None and actgrad_pre is None and drop_p == 0.0
+        C = out_view(out)
+        for b2 in range(nb2):
+            for b1 in range(nb1):
+                C[b2, b1].copy_((C[b2, b1].double() + v[b2, b1]).to(out.dtype))
+        return out
+    assert not shared, "several batch entries into one output need accumulate = 2"
+    assert not (accumulate and out.dtype == torch.bfloat16), "accumulate needs an fp32 output"
+    C = out_view(out)
     if accumulate:
         v = v + C.double()
     if bias is not None:
         assert bias.dtype == torch.float32
         v = v + bias[:N].double()
-    if bias2 is not None:  # per-utterance bias: row m takes bias2[m // bias2_rows]
-        assert nb1 == 1 and bias2.dtype == torch.float32 and bias2_rows > 0
-        v = v + bias2.double()[torch.arange(M) // bias2_rows][None, :, :N]
-    if c_pre is not None:
-        second = _gelu_grad(v) if act == "gelu_tanh_gate" else v  # ..._gate: the backward multiplier replaces the pre-activation
-        torch.as_strided(c_pre, (nb1, M, N), (c_bs[0], c_ld, 1), c_pre.storage_offset()).copy_(second.to(c_pre.dtype))
-    if act in ("gelu", "gelu_tanh", "gelu_tanh_gate"):
-        v = torch.nn.functional.gelu(v)
-    elif act == "relu":
-        v = torch.relu(v)
-    elif act == "tanh":
-        v = torch.tanh(v)
-    else:
-        assert act in (None, "none")
+    if bias2 is not None:  # per-utterance bias: row m takes bias2[m // bias2_rows], row pitch N
+        assert bias2.dtype == torch.float32 and bias2_rows > 0
+        flat = bias2.reshape(-1).double()
+        v = v + flat[(torch.arange(M) // bias2_rows)[:, None] * N + torch.arange(N)]
+    keep = gemm_keep(M, N, nb, drop_p, seed, offset).reshape(nb2, nb1, M, N) if drop_p > 0 else None
+    scale = 1.0 / (1.0 - drop_p) if drop_p > 0 else 1.0
+    if act == "gelu_tanh_gate":
+        assert c_pre is not None and out.dtype == torch.bfloat16 and N % 8 == 0
+        second = _gelu_tanh_grad(v) * (keep * scale if keep is not None else 1.0)  # the backward multiplier
+        out_view(c_pre).copy_(second.to(c_pre.dtype))
+    elif c_pre is not None:
+        out_view(c_pre).copy_(v.to(c_pre.dtype))
+    v = _act(v, act)
+    if keep is not None:
+        v = torch.where(keep, v * scale, torch.zeros_like(v))
     if actgrad_pre is not None:  # activation backward fused into the product: v *= act'(pre[m][n])
-        pre = torch.as_strided(actgrad_pre, (nb1, M, N), (c_bs[0], c_ld, 1), actgrad_pre.storage_offset()).double()
+        pre = out_view(actgrad_pre).double()
         v = v * (pre if actgrad_act == "gate" else _act_grad(pre, actgrad_act))
     if residual is not None:  # same layout and dtype as C, added after the activation
         assert residual.dtype == out.dtype
-        v = v + torch.as_strided(residual, (nb1, M, N), (c_bs[0], c_ld, 1), residual.storage_offset()).double()
+        v = v + out_view(residual).double()
     C.copy_(v.to(out.dtype))
     return out
 
@@ -98,8 +153,14 @@ def lrelu_pad(x, out, d, ph, pad, slope):
 
 
 def act_bwd(dy, pre, dpre, act, drop_p=0.0, seed=0, offset=0):
-    assert drop_p == 0.0
-    dpre.copy_((dy.double() * _act_grad(pre.double(), act)).to(dpre.dtype))
+    """st5_act_bwd: dpre = dropout-backward(dy) * act'(pre), dropout index = linear element index."""
+    g = dy.double()
+    if drop_p > 0:
+        import numpy as np
+        import dropout_ref
+        keep = torch.from_numpy(dropout_ref.keep_mask(seed, offset, np.arange(dy.numel(), dtype=np.uint64), drop_p))
+        g = torch.where(keep.reshape(dy.shape), g / (1.0 - drop_p), torch.zeros_like(g))
+    dpre.copy_((g * _act_grad(pre.double(), act)).to(dpre.dtype))
 
 
 def colsum(x2d, out, group_rows=0, accumulate=False, ld=None):
