@@ -36,6 +36,9 @@ extern "C" {
 #define ST5_ACT_GATE 5      /* actgrad_act only: actgrad_pre already holds the multiplier (written by ..._GATE below) */
 #define ST5_ACT_GELU_TANH_GATE 6 /* act only (bf16 output, N % 8 == 0, c_pre != NULL): C = dropout(gelu_tanh(x)) and c_pre
                                     receives keep * scale * gelu_tanh'(x), the factor of the FFN's dH GEMM in backward */
+#define ST5_MARGIN_NONE 0 /* speaker head: plain logits */
+#define ST5_MARGIN_AM 1   /* s (cos - m) on the margin column (AngularMargin) */
+#define ST5_MARGIN_AAM 2  /* s phi(cos) on the margin column (AdditiveAngularMargin) */
 
 int st5_version(void);
 const char* st5_last_error(void);
@@ -307,6 +310,41 @@ int st5_guided_attn_fwd(const float* const* att, int32_t n_layers, int32_t B, in
 int st5_guided_attn_bwd(float* const* datt, int32_t n_layers, int32_t B, int32_t H, int32_t heads, int32_t T_out,
                         int32_t T_in, int64_t p_ld, const int64_t* ilens, const int64_t* olens, int32_t r, float sigma,
                         float alpha, const float* gsum, const float* g, int32_t zero_rest, void* stream);
+
+/* ------------------------------------------------------------------------------------------------- speaker head
+ * Speaker identification (s2c): SpeakerDecoderPostnet (speaker_decoder_postnet.py:129-197) with its margin layers
+ * AngularMargin / AdditiveAngularMargin (speaker_decoder_postnet.py:16-126), and the s2c branch of SpeechtoTextLoss
+ * (speech_to_text_loss.py:93-110 label_smoothed_nll_loss, :340-372 compute_loss / compute_accuracy).
+ * st5_l2norm_rows_fwd: F.normalize(x, p=2, dim=1) (speaker_decoder_postnet.py:190-191): y[r] = x[r] / max(||x[r]||,
+ * 1e-12) into fp32 y [rows, E] (contiguous); nrm [rows] receives ||x[r]|| for the backward. x: row r at x + r * x_ld in
+ * `dtype`. st5_l2norm_rows_bwd: dx[r] = (dy[r] - y[r] <dy[r], y[r]>) / ||x[r]|| (dy[r] / 1e-12 on clamped rows), written
+ * in `dtype` at dx + r * dx_ld, or ADDED to it with accumulate != 0 (fp32 only: a weight gradient buffer). */
+int st5_l2norm_rows_fwd(const void* x, int64_t x_ld, int dtype, float* y, float* nrm, int64_t rows, int64_t E,
+                        void* stream);
+int st5_l2norm_rows_bwd(const float* dy, const float* y, const float* nrm, void* dx, int64_t dx_ld, int dtype,
+                        int accumulate, int64_t rows, int64_t E, void* stream);
+/* st5_margin_ce_fwd: one CTA per row b of x [B, N] fp32 (row pitch x_ld). Logits z: with mtarget == NULL, z = x; else
+ * column mtarget[b] gets the margin of `mode` (AM: s (x - m); AAM: s phi with sine = sqrt(clamp(1 - x^2, 0, 1)),
+ * phi = x cos m - sine sin m, kept where x > th = cos(pi - m) else x - mm, mm = sin(pi - m) m; easy_margin: kept where
+ * x > 0 else x, speaker_decoder_postnet.py:118-126) and every other column s x. z_out (optional, pitch z_ld) receives z.
+ * With target != NULL: log-softmax of z, then per row stats[4 b + 0..3] = label-smoothed loss (weights 1 - eps - eps_i
+ * on the target, eps_i = eps / (N - 1) on every class), nll, arg-max correct (lowest index among equal maxima), valid;
+ * all 0 on a row whose target is ignore_index. lse [B] is saved for the backward.
+ * st5_margin_ce_bwd: d z from the loss (target != NULL: gstat[0] d loss + gstat[1] d nll per valid row, both device
+ * floats) or given (dz_in, pitch dz_ld); dx [B, N] fp32 (pitch dx_ld) = d z . d z / d x, including d phi / d x on the
+ * margin column. Same margin arguments as the forward. */
+int st5_margin_ce_fwd(const float* x, int64_t x_ld, int32_t B, int32_t N, const int64_t* mtarget, int mode, float scale,
+                      float margin, int easy_margin, float* z_out, int64_t z_ld, const int64_t* target, float eps,
+                      int64_t ignore_index, float* stats, float* lse, void* stream);
+int st5_margin_ce_bwd(const float* x, int64_t x_ld, int32_t B, int32_t N, const int64_t* mtarget, int mode, float scale,
+                      float margin, int easy_margin, const int64_t* target, float eps, int64_t ignore_index,
+                      const float* lse, const float* gstat, const float* dz_in, int64_t dz_ld, float* dx, int64_t dx_ld,
+                      void* stream);
+/* st5_time_mean_fwd: y[b, c] = mean over ALL t < T of x[b, t, c] (contiguous [B, T, C] in `dtype`; the reference pools
+ * `encoder_out.transpose(0, 1).mean(1)` with padded frames included, models/speecht5.py:836-838). st5_time_mean_bwd:
+ * dx[b, t, c] = dy[b, c] / T. */
+int st5_time_mean_fwd(const void* x, void* y, int dtype, int64_t B, int64_t T, int64_t C, void* stream);
+int st5_time_mean_bwd(const void* dy, void* dx, int dtype, int64_t B, int64_t T, int64_t C, void* stream);
 
 /* ------------------------------------------------------------------------------------------------- optimizer
  * Replaces fairseq/optim/adam.py + fp16_optimizer.py:106-218 on a flat fp32 parameter buffer: one pass applies the

@@ -10,6 +10,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libspeecht5_b200.so")
 
 F32, BF16 = 0, 1
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_TANH, ACT_GELU_TANH = 0, 1, 2, 3, 4
+MARGIN_NONE, MARGIN_AM, MARGIN_AAM = 0, 1, 2  # include/speecht5_b200.h ST5_MARGIN_*
 ACT_GATE, ACT_GELU_TANH_GATE = 5, 6  # include/speecht5_b200.h ST5_ACT_GATE / ST5_ACT_GELU_TANH_GATE
 ACT_IDS = {None: ACT_NONE, "none": ACT_NONE, "relu": ACT_RELU, "gelu": ACT_GELU, "tanh": ACT_TANH,
            "gelu_tanh": ACT_GELU_TANH, "gate": ACT_GATE, "gelu_tanh_gate": ACT_GELU_TANH_GATE}
@@ -100,6 +101,14 @@ _PROTOS = {
                                       _vp]),
     "st5_guided_attn_bwd": (C.c_int, [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _i64, _vp, _vp, _i32, _f, _f, _vp, _vp,
                                       _i32, _vp]),
+    "st5_l2norm_rows_fwd": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i64, _i64, _vp]),
+    "st5_l2norm_rows_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i64, _i64, _vp]),
+    "st5_margin_ce_fwd": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _i32, _f, _f, _i32, _vp, _i64, _vp, _f, _i64, _vp, _vp,
+                                    _vp]),
+    "st5_margin_ce_bwd": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _i32, _f, _f, _i32, _vp, _f, _i64, _vp, _vp, _vp, _i64,
+                                    _vp, _i64, _vp]),
+    "st5_time_mean_fwd": (C.c_int, [_vp, _vp, _i32, _i64, _i64, _i64, _vp]),
+    "st5_time_mean_bwd": (C.c_int, [_vp, _vp, _i32, _i64, _i64, _i64, _vp]),
     "st5_sumsq": (C.c_int, [_vp, _i64, _vp, _vp]),
     "st5_adam_step": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _f, _f, _f, _f, _f, _i64, _vp, _f, _f, _vp, _vp, _vp]),
 }

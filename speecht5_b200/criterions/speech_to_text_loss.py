@@ -100,7 +100,33 @@ class SpeechtoTextLoss(FairseqCriterion):
                               reduction="sum", zero_infinity=self.zero_infinity)
         return loss, lprobs, input_lengths
 
+    # ------------------------------------------------------------------ speaker identification (s2c)
+    def _forward_s2c(self, model, sample):
+        """speecht5_criterion.py:113 sends s2c here: the model returns ((class logits [B, N], embedding), None) and the
+        loss is the label-smoothed CE of compute_loss on target [B, 1], with compute_accuracy's counts; one row kernel
+        (csrc/speaker_head.cu) computes all of it. The speaker model has no CTC head."""
+        from .. import ops
+        if self.ctc_weight > 0 or self.ce_weight <= 0:
+            raise NotImplementedError("speaker identification is trained with cross entropy only (ctc_weight 0)")
+        (logits, _), _ = model(**sample["net_input"])
+        sums = ops.margin_ce(logits, sample["target"], self.eps, self.padding_idx)  # loss, nll, n_correct, total
+        loss, nll = sums[0], sums[1]
+        ntokens = sample["ntokens"] if "ntokens" in sample else int(sample["target_lengths"].sum().item())
+        sample_size = sample["target"].size(0) if self.sentence_avg else ntokens
+        nsent = sample["target"].size(0)
+        if getattr(self, "defer_logging", False):
+            stats = torch.stack([loss.detach(), loss.detach(), loss.new_zeros(()), nll.detach(), sums[2], sums[3]])
+            return loss, sample_size, {"_stats": stats, "ntokens": ntokens, "nsentences": nsent,
+                                       "sample_size": sample_size}
+        log = {"loss": loss.item(), "ce_loss": loss.item(), "ctc_loss": 0, "nll_loss": nll.item(), "ntokens": ntokens,
+               "nsentences": nsent, "sample_size": sample_size}
+        if self.report_accuracy:
+            log["n_correct"], log["total"] = int(sums[2].item()), int(sums[3].item())
+        return loss, sample_size, log
+
     def forward(self, model, sample, reduce=True):
+        if sample.get("task_name") == "s2c" and getattr(model, "speaker_decoder_postnet", None) is not None:
+            return self._forward_s2c(model, sample)
         if self.ce_weight == 0 and self.ctc_weight > 0:
             sample["only_ctc"] = True  # (:189-190; as in the reference this key never reaches the model call)
         net_output_decoder, net_output = model(**sample["net_input"])

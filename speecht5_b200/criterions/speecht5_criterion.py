@@ -1,5 +1,5 @@
 """@register_criterion("speecht5") dispatcher, mirroring speecht5/criterions/speecht5_criterion.py:23-120: routes on
-sample['task_name'] to the t2s / s2s (TexttoSpeechLoss), s2t (SpeechtoTextLoss), text_pretrain and speech_pretrain
+sample['task_name'] to the t2s / s2s (TexttoSpeechLoss), s2t and s2c (SpeechtoTextLoss), text_pretrain and speech_pretrain
 criteria; note the reference dispatcher does not forward guided_attn_loss_lambda, so the effective guided-attention
 weight is 1.0 (speecht5_criterion.py:61-71)."""
 import math
@@ -17,7 +17,7 @@ from .text_to_speech_loss import TexttoSpeechLoss
 class SpeechT5CriterionConfig:
     """Union of the reference's criterion configs (speecht5_criterion.py:23-30 inherits the text-to-speech,
     speech-to-text, label-smoothed CE and pre-training configs), so every recipe's `--criterion speecht5 ...` flags
-    parse. Fields of branches that are not built (speaker identification) are accepted and only matter once that branch is called."""
+    parse."""
     sentence_avg: bool = field(default=True)
     # text_to_speech_loss.py:21-69
     use_masking: bool = field(default=True)
@@ -74,13 +74,13 @@ class SpeechT5Criterion(FairseqCriterion):
         task_name = sample["task_name"]
         if task_name in ("t2s", "s2s"):
             return self.text_to_speech_loss(model, sample)
-        if task_name == "s2t":
+        if task_name in ("s2t", "s2c"):  # (:113: speaker identification is CE on the class logits)
             return self.speech_to_text_loss(model, sample, reduce)
         if task_name == "text_pretrain":
             return self.text_pretrain_criterion(model, sample, reduce)
         if task_name == "speech_pretrain":
             return self.speech_pretrain_criterion(model, sample, reduce)
-        raise NotImplementedError(f"criterion branch '{task_name}' is not built in the H100 path (speaker identification)")
+        raise NotImplementedError(f"criterion branch '{task_name}' is not built in the H100 path")
 
     # ------------------------------------------------------------------ logging (speecht5_criterion.py:123-436)
     @staticmethod

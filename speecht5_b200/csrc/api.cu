@@ -233,6 +233,37 @@ int st5_ctc_loss(const float* logits, int64_t ld_t, int64_t ld_b, const int64_t*
                    "st5_ctc_loss");
 }
 
+int st5_l2norm_rows_fwd(const void* x, int64_t x_ld, int dtype, float* y, float* nrm, int64_t rows, int64_t E,
+                        void* stream) {
+  return set_error(l2norm_rows_fwd_launch(x, x_ld, dtype, y, nrm, rows, E, (cudaStream_t)stream), "st5_l2norm_rows_fwd");
+}
+int st5_l2norm_rows_bwd(const float* dy, const float* y, const float* nrm, void* dx, int64_t dx_ld, int dtype,
+                        int accumulate, int64_t rows, int64_t E, void* stream) {
+  return set_error(l2norm_rows_bwd_launch(dy, y, nrm, dx, dx_ld, dtype, accumulate, rows, E, (cudaStream_t)stream),
+                   "st5_l2norm_rows_bwd");
+}
+int st5_margin_ce_fwd(const float* x, int64_t x_ld, int32_t B, int32_t N, const int64_t* mtarget, int mode, float scale,
+                      float margin, int easy_margin, float* z_out, int64_t z_ld, const int64_t* target, float eps,
+                      int64_t ignore_index, float* stats, float* lse, void* stream) {
+  return set_error(margin_ce_fwd_launch(x, x_ld, B, N, mtarget, mode, scale, margin, easy_margin, z_out, z_ld, target,
+                                        eps, ignore_index, stats, lse, (cudaStream_t)stream),
+                   "st5_margin_ce_fwd");
+}
+int st5_margin_ce_bwd(const float* x, int64_t x_ld, int32_t B, int32_t N, const int64_t* mtarget, int mode, float scale,
+                      float margin, int easy_margin, const int64_t* target, float eps, int64_t ignore_index,
+                      const float* lse, const float* gstat, const float* dz_in, int64_t dz_ld, float* dx, int64_t dx_ld,
+                      void* stream) {
+  return set_error(margin_ce_bwd_launch(x, x_ld, B, N, mtarget, mode, scale, margin, easy_margin, target, eps,
+                                        ignore_index, lse, gstat, dz_in, dz_ld, dx, dx_ld, (cudaStream_t)stream),
+                   "st5_margin_ce_bwd");
+}
+int st5_time_mean_fwd(const void* x, void* y, int dtype, int64_t B, int64_t T, int64_t C, void* stream) {
+  return set_error(time_mean_fwd_launch(x, y, dtype, B, T, C, (cudaStream_t)stream), "st5_time_mean_fwd");
+}
+int st5_time_mean_bwd(const void* dy, void* dx, int dtype, int64_t B, int64_t T, int64_t C, void* stream) {
+  return set_error(time_mean_bwd_launch(dy, dx, dtype, B, T, C, (cudaStream_t)stream), "st5_time_mean_bwd");
+}
+
 int st5_sumsq(const float* x, int64_t n, float* out, void* stream) {
   return set_error(sumsq_launch(x, n, out, (cudaStream_t)stream), "st5_sumsq");
 }

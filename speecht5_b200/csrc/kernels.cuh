@@ -188,6 +188,19 @@ int ctc_loss_launch(const float* logits, int64_t ld_t, int64_t ld_b, const int64
                     const int64_t* input_lengths, const int64_t* target_lengths, float* nll, float* grad, float* ws,
                     int32_t T, int32_t B, int32_t V, int32_t S_max, int32_t blank, int32_t zero_infinity,
                     cudaStream_t s);
+int l2norm_rows_fwd_launch(const void* x, int64_t x_ld, int dtype, float* y, float* nrm, int64_t rows, int64_t E,
+                           cudaStream_t s);
+int l2norm_rows_bwd_launch(const float* dy, const float* y, const float* nrm, void* dx, int64_t dx_ld, int dtype,
+                           int accumulate, int64_t rows, int64_t E, cudaStream_t s);
+int margin_ce_fwd_launch(const float* x, int64_t x_ld, int32_t B, int32_t N, const int64_t* mtarget, int mode,
+                         float scale, float margin, int easy, float* z_out, int64_t z_ld, const int64_t* target,
+                         float eps, int64_t ignore_index, float* stats, float* lse, cudaStream_t s);
+int margin_ce_bwd_launch(const float* x, int64_t x_ld, int32_t B, int32_t N, const int64_t* mtarget, int mode,
+                         float scale, float margin, int easy, const int64_t* target, float eps, int64_t ignore_index,
+                         const float* lse, const float* gstat, const float* dz_in, int64_t dz_ld, float* dx,
+                         int64_t dx_ld, cudaStream_t s);
+int time_mean_fwd_launch(const void* x, void* y, int dtype, int64_t B, int64_t Tn, int64_t C, cudaStream_t s);
+int time_mean_bwd_launch(const void* dy, void* dx, int dtype, int64_t B, int64_t Tn, int64_t C, cudaStream_t s);
 int sumsq_launch(const float* x, int64_t n, float* out, cudaStream_t s);
 int adam_launch(float* p, const float* g, float* m, float* v, void* p_bf16, int64_t n, float lr, float beta1,
                 float beta2, float eps, float weight_decay, int64_t step, const float* grad_norm_sq, float max_norm,

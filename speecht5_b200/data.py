@@ -146,13 +146,7 @@ def collate_asr(samples, pad=1, eos=2):
     samples = [s for s in samples if s["source"] is not None]
     if len(samples) == 0:
         return {}
-    audios = [s["source"] for s in samples]
-    n = max(len(a) for a in audios)
-    source = audios[0].new_zeros(len(audios), n)
-    padding_mask = torch.zeros(len(audios), n, dtype=torch.bool)
-    for i, a in enumerate(audios):
-        source[i, : len(a)] = a
-        padding_mask[i, len(a):] = True
+    source, padding_mask = _collate_audio([s["source"] for s in samples])
     labels = [torch.cat((s["label_list"][0].long(), torch.tensor([eos]))) for s in samples]
     lengths = torch.tensor([len(t) for t in labels], dtype=torch.long)
     T = int(lengths.max())
@@ -167,6 +161,47 @@ def collate_asr(samples, pad=1, eos=2):
             "net_input": {"source": source, "padding_mask": padding_mask, "prev_output_tokens": prev,
                           "task_name": "s2t"},
             "target": target, "target_lengths": lengths, "task_name": "s2t", "ntokens": ntokens}
+
+
+def _collate_audio(audios):
+    """Zero-padded waveforms [B, n_max] and their boolean padding mask (True on padding)."""
+    n = max(len(a) for a in audios)
+    source = audios[0].new_zeros(len(audios), n)
+    padding_mask = torch.zeros(len(audios), n, dtype=torch.bool)
+    for i, a in enumerate(audios):
+        source[i, : len(a)] = a
+        padding_mask[i, len(a):] = True
+    return source, padding_mask
+
+
+def collate_sid(samples, pad=1, eos=2):
+    """SpeechToClassDataset.collater (speecht5/data/speech_to_class_dataset.py:138-198) over in-memory items
+    {"id", "source": FloatTensor [N] waveform, "label": class index}: zero-padded waveforms with their padding mask,
+    target [B, 1] (collate_tokens of one-token labels: no eos), prev_output_tokens [[eos]] per utterance, ntokens = B."""
+    samples = [s for s in samples if s["source"] is not None]
+    if len(samples) == 0:
+        return {}
+    source, padding_mask = _collate_audio([s["source"] for s in samples])
+    B = len(samples)
+    target = torch.tensor([[int(s["label"])] for s in samples], dtype=torch.long)
+    return {"id": torch.LongTensor([s["id"] for s in samples]),
+            "net_input": {"source": source, "padding_mask": padding_mask,
+                          "prev_output_tokens": torch.full((B, 1), eos, dtype=torch.long), "task_name": "s2c"},
+            "target": target, "target_lengths": torch.ones(B, dtype=torch.long), "task_name": "s2c", "ntokens": B}
+
+
+def synthetic_sid_batch(B, n_samples, n_classes, seed=1, ragged=True, pin=False):
+    """Speaker-identification batch through the s2c collater: waveforms N(0, 0.1^2) with lengths U{0.8 n .. n} (the
+    first one n), speakers U{4 .. n_classes - 3} (the dictionary's specials and its trailing <mask> / <ctc_blank> are
+    never a class)."""
+    g = torch.Generator().manual_seed(seed)
+    items = []
+    for b in range(B):
+        n = n_samples if (b == 0 or not ragged) else int(torch.randint(int(0.8 * n_samples), n_samples + 1, (1,), generator=g))
+        items.append({"id": b, "source": torch.randn(n, generator=g) * 0.1,
+                      "label": int(torch.randint(4, n_classes - 2, (1,), generator=g))})
+    sample = collate_sid(items)
+    return _pin(sample) if pin else sample
 
 
 def _span_lengths(rng, kind, count, length, other):

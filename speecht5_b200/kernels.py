@@ -412,6 +412,80 @@ def guided_attn_bwd(datts, heads, T_in, ilens, olens, r, sigma, alpha, gsum, g, 
     _count(1)
 
 
+def l2norm_rows_fwd(x, y, nrm):
+    """st5_l2norm_rows_fwd: y [rows, E] fp32 = F.normalize(x, dim=1); nrm [rows] = row norms. x: 2-D, unit inner stride."""
+    _require_cuda(x, y, nrm)
+    rows, E = x.shape
+    assert x.stride(1) == 1 and y.dtype == torch.float32 and y.is_contiguous() and y.shape == (rows, E)
+    _lib.check(_lib.load().st5_l2norm_rows_fwd(_ptr(x), x.stride(0), dtype_id(x), _ptr(y), _ptr(nrm), rows, E,
+                                               _stream()), "st5_l2norm_rows_fwd")
+    _count(1)
+
+
+def l2norm_rows_bwd(dy, y, nrm, dx, accumulate=False):
+    """st5_l2norm_rows_bwd: dx (2-D, unit inner stride; fp32 when accumulate) <- (or +=) the input gradient."""
+    _require_cuda(dy, y, nrm, dx)
+    rows, E = y.shape
+    assert dy.dtype == torch.float32 and dy.is_contiguous() and dx.stride(1) == 1 and dx.shape == (rows, E)
+    _lib.check(_lib.load().st5_l2norm_rows_bwd(_ptr(dy), _ptr(y), _ptr(nrm), _ptr(dx), dx.stride(0), dtype_id(dx),
+                                               int(accumulate), rows, E, _stream()), "st5_l2norm_rows_bwd")
+    _count(1)
+
+
+def _margin_args(margin):
+    """margin: None or (mode, scale, m, easy_margin)."""
+    return (_lib.MARGIN_NONE, 1.0, 0.0, 0) if margin is None else (int(margin[0]), float(margin[1]),
+                                                                  float(margin[2]), int(margin[3]))
+
+
+def margin_ce_fwd(x, mtarget, margin, z_out=None, target=None, eps=0.0, ignore_index=-100, stats=None, lse=None):
+    """st5_margin_ce_fwd over x [B, N] fp32 (unit inner stride): margin logits into z_out and / or per-row (loss, nll,
+    correct, valid) into stats [B, 4] with lse [B] for the backward."""
+    _require_cuda(x, z_out, target, stats, lse)
+    B, N = x.shape
+    assert x.dtype == torch.float32 and x.stride(1) == 1
+    for t in (mtarget, target):
+        assert t is None or (t.dtype == torch.int64 and t.is_contiguous() and t.numel() == B)
+    assert z_out is None or (z_out.dtype == torch.float32 and z_out.stride(1) == 1)
+    mode, s, m, easy = _margin_args(margin)
+    _lib.check(_lib.load().st5_margin_ce_fwd(_ptr(x), x.stride(0), B, N, _ptr(mtarget), mode, s, m, easy, _ptr(z_out),
+                                             z_out.stride(0) if z_out is not None else 0, _ptr(target), eps,
+                                             ignore_index, _ptr(stats), _ptr(lse), _stream()), "st5_margin_ce_fwd")
+    _count(1)
+
+
+def margin_ce_bwd(x, mtarget, margin, dx, target=None, eps=0.0, ignore_index=-100, lse=None, gstat=None, dz=None):
+    """st5_margin_ce_bwd: dx [B, N] fp32 = d logits from the loss (target, lse, gstat [2] device floats) or from dz."""
+    _require_cuda(x, dx, dz)
+    B, N = x.shape
+    assert dx.dtype == torch.float32 and dx.stride(1) == 1
+    assert gstat is None or (gstat.dtype == torch.float32 and gstat.is_contiguous())
+    assert dz is None or (dz.dtype == torch.float32 and dz.stride(1) == 1)
+    mode, s, m, easy = _margin_args(margin)
+    _lib.check(_lib.load().st5_margin_ce_bwd(_ptr(x), x.stride(0), B, N, _ptr(mtarget), mode, s, m, easy, _ptr(target),
+                                             eps, ignore_index, _ptr(lse), _ptr(gstat), _ptr(dz),
+                                             dz.stride(0) if dz is not None else 0, _ptr(dx), dx.stride(0), _stream()),
+               "st5_margin_ce_bwd")
+    _count(1)
+
+
+def time_mean_fwd(x, y):
+    """st5_time_mean_fwd: y [B, C] = x [B, T, C].mean(1) (contiguous, one dtype)."""
+    _require_cuda(x, y)
+    B, T, Cc = x.shape
+    assert x.is_contiguous() and y.is_contiguous() and x.dtype == y.dtype and y.shape == (B, Cc)
+    _lib.check(_lib.load().st5_time_mean_fwd(_ptr(x), _ptr(y), dtype_id(x), B, T, Cc, _stream()), "st5_time_mean_fwd")
+    _count(1)
+
+
+def time_mean_bwd(dy, dx):
+    _require_cuda(dy, dx)
+    B, T, Cc = dx.shape
+    assert dy.is_contiguous() and dx.is_contiguous() and dy.dtype == dx.dtype
+    _lib.check(_lib.load().st5_time_mean_bwd(_ptr(dy), _ptr(dx), dtype_id(dx), B, T, Cc, _stream()), "st5_time_mean_bwd")
+    _count(1)
+
+
 def sumsq(x, out):
     lib = _lib.load()
     _lib.check(lib.st5_sumsq(_ptr(x), x.numel(), _ptr(out), _stream()), "st5_sumsq")

@@ -5,9 +5,10 @@ t5_transformer_base, t5_transformer_large, t5_transformer_base_asr :1252,1385,14
 
 Coverage of forward(): text -> speech (t2s, the BASELINE.json metric path), speech -> text (s2t: waveform front end,
 CE + CTC), text -> text (t2t / text pre-training), speech pre-training (HuBERT targets, masked-prediction head, shared
-Gumbel quantizer, reconstruction through the speech decoder; only_hubert / feature_only returns), greedy generation of
-speech and text. The branches SURVEY.md section 2 leaves out (speaker identification s2c, voice conversion /
-enhancement s2s inputs) raise NotImplementedError rather than silently falling back to PyTorch."""
+Gumbel quantizer, reconstruction through the speech decoder; only_hubert / feature_only returns), speaker
+identification (s2c: speaker head on the pooled decoder or encoder state, margin softmax), greedy generation of speech
+and text, class prediction. The branches SURVEY.md section 2 leaves out (voice conversion / enhancement s2s inputs)
+raise NotImplementedError rather than silently falling back to PyTorch."""
 import argparse
 import logging
 from argparse import Namespace
@@ -17,7 +18,9 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..fairseq_shim import FairseqEncoderDecoderModel, register_model, register_model_architecture
+from .. import ops
 from ..ops import RT
+from .modules.speaker_decoder_postnet import SpeakerDecoderPostnet
 from .modules.nets import (SpeechDecoderPostnet, SpeechDecoderPrenet, TextDecoderPostnet, TextDecoderPrenet,
                            TextEncoderPrenet)
 from .modules.transformer import MultiheadAttention, TransformerDecoder, TransformerEncoder
@@ -175,9 +178,10 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
         ("--conv-pos", dict(type=int)),
         ("--conv-pos-groups", dict(type=int)),
         ("--get-code-distribution", dict(action="store_true")),
-        # options of branches this implementation does not build (speaker identification, enhancement, the
-        # convolutional subsampler, sliding-window / branched encoders): accepted so that every recipe's command line
-        # parses; they only matter once such a branch is called, and those raise NotImplementedError
+        # options of branches this implementation does not build (enhancement, the convolutional subsampler,
+        # sliding-window / branched encoders, the speaker-identification variants _check_sid_options lists): accepted so
+        # that every recipe's command line parses; they only matter once such a branch is called or built, and those
+        # raise NotImplementedError
         ("--encoder-sliding-window-attn", dict(type=int, default=None)),
         ("--conv-kernel-sizes", dict(type=str, default="5,5")),
         ("--conv-channels", dict(type=int, default=1024)),
@@ -259,8 +263,14 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
                 logit_temp=getattr(args, "logit_temp", 0.1), untie_final_proj=getattr(args, "untie_final_proj", True),
                 skip_masked=getattr(args, "skip_masked", False), skip_nomask=getattr(args, "skip_nomask", False),
                 target_glu=getattr(args, "target_glu", False))
+        # speaker-identification head (:709-715): one class per entry of the task's text dictionary
+        speaker_decoder_postnet = None
+        if getattr(task, "t5_task", None) == "s2c":
+            _check_sid_options(args)
+            speaker_decoder_postnet = SpeakerDecoderPostnet(args.sid_embed_dim, len(text_dict), args)
         return cls(args, encoder, decoder, text_encoder_prenet, speech_encoder_prenet, text_decoder_prenet,
-                   speech_decoder_prenet, text_decoder_postnet, speech_decoder_postnet, None, speech_encoder_postnet)
+                   speech_decoder_prenet, text_decoder_postnet, speech_decoder_postnet, speaker_decoder_postnet,
+                   speech_encoder_postnet)
 
     # ------------------------------------------------------------------ forward (models/speecht5.py:786-963)
     def forward(self, source=None, src_tokens=None, src_lengths=None, prev_output_tokens=None, tgt_lengths=None,
@@ -269,6 +279,9 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
         """Reference signature (:786) + two optional extras: `mask_indices` / `mask_channel_indices`, a HuBERT-style mask
         draw made by the caller (the trainer draws on the host before replaying a captured step)."""
         assert source is not None or src_tokens is not None
+        if task_name == "s2c" and self.speaker_decoder_postnet is not None:
+            return self._forward_s2c(source, padding_mask, prev_output_tokens, target_list, mask, mask_indices,
+                                     mask_channel_indices)
         input_type = "text" if (source is None and padding_mask is None and not feature_only) else "speech"
         output_type = "text" if (prev_output_tokens is not None and prev_output_tokens.dim() == 2) else "speech"
         text_out = output_type == "text" and self.text_decoder_prenet is not None
@@ -346,6 +359,47 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
         if target_list is not None:  # (:960-961) speech pre-training: head results + the reconstruction branch
             return hubert_results, (self.speech_decoder_postnet(decoder_output) + (extra["attn"][0],))
         return self.speech_decoder_postnet(decoder_output) + (extra["attn"][0],)
+
+    def _forward_s2c(self, source, padding_mask, prev_output_tokens, target_list, mask, mask_indices,
+                     mask_channel_indices):
+        """Speaker identification (:805-810, 836-838, 896-897, 925-928): waveform -> encoder; pooling "encoder" averages
+        ALL encoder frames (padding included, as the reference's `.mean(1)` does), pooling "decoder" runs the decoder on
+        one zero query row [B, 1, C] against the encoder states. The head's margin goes to the class in `target_list`
+        ([B, 1] class indices) in training. Returns ((logits, embedding), None)."""
+        if source is None or self.speech_encoder_prenet is None:
+            raise NotImplementedError("speaker identification takes a waveform (--build-speech-encoder)")
+        sid_target = None
+        if target_list is not None and target_list.dim() == 2 and target_list.size(1) == 1:
+            sid_target = target_list[:, 0]
+        encoder_input, encoder_padding_mask = self.speech_encoder_prenet(
+            source, padding_mask=padding_mask, mask=self.training and mask, mask_indices=mask_indices,
+            mask_channel_indices=mask_channel_indices)
+        encoder_output = self.encoder(encoder_input, encoder_padding_mask)
+        if self.args.sid_pooling_layer == "encoder":
+            return self.speaker_decoder_postnet(ops.time_mean(encoder_output["_encoder_out_btc"]), sid_target), None
+        if "decoder_input" in encoder_output and encoder_output["decoder_input"][0] is not None:  # (:854-856)
+            encoder_output["encoder_out"] = encoder_output["decoder_input"]
+            encoder_output["_encoder_out_btc"] = encoder_output["decoder_input"][0].transpose(0, 1)
+        return self.speaker_decoder_postnet(self._decoder_pool(prev_output_tokens, encoder_output), sid_target), None
+
+    def _decoder_pool(self, prev_output_tokens, encoder_output):
+        """The decoder on a zero [B, 1, C] query (the s2c [CLS] vector, :896-897 / :1174-1175); its single output row."""
+        if prev_output_tokens is None or prev_output_tokens.dim() != 2 or prev_output_tokens.size(1) != 1:
+            raise ValueError("speaker identification feeds the decoder one query token per utterance: "
+                             "prev_output_tokens [B, 1] (the s2c collater's [[eos]])")
+        dec_in, tgt_mask, _ = self.text_decoder_prenet(prev_output_tokens)
+        decoder_output, _ = self.decoder(torch.zeros_like(dec_in), tgt_mask, encoder_output, alignment_layer=None)
+        return decoder_output[:, 0]
+
+    @torch.no_grad()
+    def generate_class(self, source, prev_output_tokens, **kwargs):
+        """models/speecht5.py:1171-1186 (what scripts/generate_class.py calls through the task): the arg-max class of
+        the head on the DECODER output, whatever --sid-pooling-layer says (the reference's own quirk), no margin."""
+        if self.speaker_decoder_postnet is None:
+            raise NotImplementedError("generate_class needs the speaker head: build the model for t5_task s2c")
+        encoder_out = self.forward_encoder(source, padding_mask=kwargs.get("padding_mask"))
+        output, _ = self.speaker_decoder_postnet(self._decoder_pool(prev_output_tokens, encoder_out))
+        return output.argmax(1)
 
     # ------------------------------------------------------------------ fairseq model API used by callers
     def set_num_updates(self, num_updates):
@@ -654,6 +708,13 @@ def base_architecture(args):  # models/speecht5.py:1252-1383 (fields used by the
     g("use_conv_pos", False)
     g("use_sinc_pos", False)
     g("encoder_speech_prenet", "conv")
+    # speaker identification (:1273-1275, :1327-1331)
+    g("decoder_output_dim", args.decoder_embed_dim)
+    g("sid_embed_dim", 128)
+    g("sid_pooling_layer", "decoder")
+    g("softmax_scale", 1)
+    g("softmax_margin", 0)
+    g("softmax_easy_margin", False)
 
 
 @register_model_architecture("t5_transformer", "t5_transformer_base")
@@ -718,6 +779,19 @@ def t5_transformer_base_asr(args):  # :1427-1447
     g("use_sinc_pos", True)
     g("max_text_positions", 600)
     base_architecture(args)
+
+
+def _check_sid_options(args):
+    """The speaker-identification variants that are not built fail at build time rather than at the first batch."""
+    if getattr(args, "sid_pooling_layer", "decoder") not in ("decoder", "encoder"):
+        raise NotImplementedError(f"--sid-pooling-layer {args.sid_pooling_layer}: only 'decoder' and 'encoder' are built")
+    for opt in ("sid_t5_postnet", "sid_encoder_cls", "sid_shuffle_encoder_input", "sid_decoder_speaker", "sid_pad_prenet"):
+        if getattr(args, opt, None):
+            raise NotImplementedError(f"--{opt.replace('_', '-')} is not built for speaker identification")
+    if getattr(args, "use_codebook", False):
+        raise NotImplementedError("speaker identification with --use-codebook is not built")
+    if not (getattr(args, "build_speech_encoder", False) and getattr(args, "build_text_decoder", False)):
+        raise NotImplementedError("speaker identification needs --build-speech-encoder and --build-text-decoder")
 
 
 def make_args(arch="t5_transformer_base_asr", **overrides):

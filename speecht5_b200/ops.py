@@ -937,7 +937,9 @@ class AttentionTCFn(torch.autograd.Function):
             with_pe = pe_k is not None
             pe_hi = _pe_bf16(pe_k) if with_pe else None
             probs = torch.empty((B, H, Tq, p_ld), dtype=torch.float32, device=dev) if want else None
-            grad = any(ctx.needs_input_grad[:3])  # (inference: nothing is saved, the kernel skips those stores)
+            # (inference: nothing is saved, the kernel skips those stores. needs_input_grad alone is not enough: under
+            # torch.no_grad it still reports the relative-position table, a parameter)
+            grad = cfg.get("grad_enabled", True) and any(ctx.needs_input_grad[:3])
             psave = torch.empty((B, H, Tq, p_ld), dtype=torch.bfloat16, device=dev) if grad else None
             inv_l = torch.empty((B, H, Tq), dtype=torch.float32, device=dev) if grad else None
             o32 = torch.empty((B, Tq, d), dtype=torch.float32, device=dev) if grad else None
@@ -1059,7 +1061,7 @@ def attention(q_buf, kv_buf, *, H, d, q_col, k_col, v_col, scale, pe_k=None, max
     # guided-attention loss; set by the trainer from the criterion): the backward skips the zero gradient of the others
     cfg = dict(H=H, d=d, q_col=q_col, k_col=k_col, v_col=v_col, scale=scale, maxpos=maxpos, causal=causal,
                drop_p=drop_p, return_probs=return_probs, probs_grad_heads=RT.probs_grad_heads if return_probs else 0,
-               probs_read_heads=RT.probs_read_heads if return_probs else 0)
+               probs_read_heads=RT.probs_read_heads if return_probs else 0, grad_enabled=torch.is_grad_enabled())
     Tk = (q_buf if kv_buf is None else kv_buf).shape[1]
     streaming = RT.attn_flash and RT.attn_fused and RT.attn_fused_bwd and (pe_k is None or not causal)
     if q_buf.dtype == torch.bfloat16 and RT.attn_tensor_core and (Tk <= 512 or streaming):
@@ -1238,3 +1240,175 @@ def dropout(x, drop_p, training=True):
     if drop_p <= 0.0 or not training:
         return x
     return DropoutFn.apply(x, drop_p)
+
+
+# =================================================================================================== speaker head
+def _operands(x):
+    """fp32 [rows, cols] (unit inner stride) -> GEMM operands in padded rows: the (hi, lo) bf16 split in parity mode,
+    (hi, None) in throughput mode."""
+    rows, cols = x.shape
+    pair = torch.empty((2 if RT.dtype == torch.float32 else 1, rows, _pad8(cols)), dtype=torch.bfloat16, device=x.device)
+    hi = pair[0, :, :cols]
+    lo = pair[1, :, :cols] if pair.shape[0] == 2 else None
+    K.cast_bf16(x, hi, lo)
+    return hi, lo
+
+
+def _padded_f32(t):
+    """fp32 view with unit inner stride and a 16-byte aligned row pitch (what the GEMM and row kernels read)."""
+    t = t.float()
+    if t.stride(1) == 1 and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0:
+        return t
+    buf = torch.empty((t.shape[0], _pad8(t.shape[1])), dtype=torch.float32, device=t.device)[:, :t.shape[1]]
+    buf.copy_(t)
+    return buf
+
+
+class L2NormRowsFn(torch.autograd.Function):
+    """F.normalize(x, p=2, dim=1) (speaker_decoder_postnet.py:190-191) -> fp32 rows. grad_key: the trainer's flat
+    gradient view the input gradient is accumulated into (the class weight), if one is registered."""
+
+    @staticmethod
+    def forward(ctx, x, grad_key):
+        x2 = x if x.stride(-1) == 1 else x.contiguous()
+        y = torch.empty(x2.shape, dtype=torch.float32, device=x.device)
+        nrm = torch.empty(x2.shape[0], dtype=torch.float32, device=x.device)
+        K.l2norm_rows_fwd(x2, y, nrm)
+        ctx.save_for_backward(y, nrm)
+        ctx.meta = (x.dtype, grad_key)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        y, nrm = ctx.saved_tensors
+        dtype, grad_key = ctx.meta
+        dy = dy.float().contiguous()
+        target = RT._static_grad.get(grad_key) if grad_key is not None else None
+        if target is not None:
+            K.l2norm_rows_bwd(dy, y, nrm, target, accumulate=True)
+            return None, None
+        dx = torch.empty(y.shape, dtype=dtype, device=y.device)
+        K.l2norm_rows_bwd(dy, y, nrm, dx)
+        return dx, None
+
+
+def l2_normalize_rows(x, grad_key=None):
+    return L2NormRowsFn.apply(x, grad_key)
+
+
+class CosineFn(torch.autograd.Function):
+    """out [B, N] fp32 = xn . wn^T (F.linear(x_norm, w_norm), speaker_decoder_postnet.py:192) and its two gradient
+    GEMMs on the wgmma kernel; parity mode contracts the hi/lo splits."""
+
+    @staticmethod
+    def forward(ctx, xn, wn):
+        B, E = xn.shape
+        N = wn.shape[0]
+        ldc = _pad8(N)
+        out = torch.empty((B, ldc), dtype=torch.float32, device=xn.device)
+        xa, wa = _operands(xn), _operands(wn)
+        mm(xa, wa, out, M=B, N=N, Kd=E, a_ld=xa[0].stride(0), b_ld=wa[0].stride(0), c_ld=ldc)
+        ctx.ops = (xa, wa)
+        return out[:, :N]
+
+    @staticmethod
+    def backward(ctx, dc):
+        xa, wa = ctx.ops
+        B, E = xa[0].shape
+        N = wa[0].shape[0]
+        ga = _operands(_padded_f32(dc))
+        dxn = dwn = None
+        if ctx.needs_input_grad[0]:
+            dxn = torch.empty((B, E), dtype=torch.float32, device=dc.device)
+            mm(ga, wa, dxn, M=B, N=E, Kd=N, a_ld=ga[0].stride(0), b_mn=True, b_ld=wa[0].stride(0), c_ld=E)
+        if ctx.needs_input_grad[1]:
+            dwn = torch.empty((N, E), dtype=torch.float32, device=dc.device)
+            mm(ga, xa, dwn, M=N, N=E, Kd=B, a_mn=True, a_ld=ga[0].stride(0), b_mn=True, b_ld=xa[0].stride(0), c_ld=E)
+        return dxn, dwn
+
+
+def cosine(xn, wn):
+    return CosineFn.apply(xn, wn)
+
+
+class MarginFn(torch.autograd.Function):
+    """AngularMargin / AdditiveAngularMargin (speaker_decoder_postnet.py:48-126) on the cosines with the margin on
+    column mtarget[b] of row b; margin = (mode, scale, m, easy_margin)."""
+
+    @staticmethod
+    def forward(ctx, cos, mtarget, margin):
+        cos = _padded_f32(cos)
+        B, N = cos.shape
+        z = torch.empty((B, _pad8(N)), dtype=torch.float32, device=cos.device)[:, :N]
+        K.margin_ce_fwd(cos, mtarget, margin, z_out=z)
+        ctx.save_for_backward(cos, mtarget)
+        ctx.margin = margin
+        return z
+
+    @staticmethod
+    def backward(ctx, dz):
+        cos, mtarget = ctx.saved_tensors
+        B, N = cos.shape
+        dx = torch.empty((B, _pad8(N)), dtype=torch.float32, device=cos.device)[:, :N]
+        K.margin_ce_bwd(cos, mtarget, ctx.margin, dx, dz=_padded_f32(dz))
+        return dx, None, None
+
+
+def margin_logits(cos, mtarget, margin):
+    return MarginFn.apply(cos, mtarget.contiguous(), margin)
+
+
+class MarginCEFn(torch.autograd.Function):
+    """Label-smoothed cross entropy of SpeechtoTextLoss on class logits [B, N] (speech_to_text_loss.py:93-110, 340-372)
+    in one row kernel: returns the sums (loss, nll, n_correct, total) over the rows; only loss and nll carry gradient."""
+
+    @staticmethod
+    def forward(ctx, z, target, eps, ignore_index):
+        z = _padded_f32(z)
+        B, N = z.shape
+        stats = torch.empty((B, 4), dtype=torch.float32, device=z.device)
+        lse = torch.empty(B, dtype=torch.float32, device=z.device)
+        target = target.reshape(-1).contiguous()
+        K.margin_ce_fwd(z, None, None, target=target, eps=eps, ignore_index=ignore_index, stats=stats, lse=lse)
+        sums = torch.empty(4, dtype=torch.float32, device=z.device)
+        K.colsum(stats, sums)
+        ctx.save_for_backward(z, target, lse)
+        ctx.meta = (eps, ignore_index)
+        return sums
+
+    @staticmethod
+    def backward(ctx, g):
+        z, target, lse = ctx.saved_tensors
+        eps, ignore_index = ctx.meta
+        B, N = z.shape
+        dz = torch.empty((B, _pad8(N)), dtype=torch.float32, device=z.device)[:, :N]
+        K.margin_ce_bwd(z, None, None, dz, target=target, eps=eps, ignore_index=ignore_index, lse=lse,
+                        gstat=g.float().contiguous())
+        return dz, None, None, None
+
+
+def margin_ce(z, target, eps, ignore_index):
+    return MarginCEFn.apply(z, target, eps, ignore_index)
+
+
+class TimeMeanFn(torch.autograd.Function):
+    """x [B, T, C] -> mean over all T frames (padding included, models/speecht5.py:838)."""
+
+    @staticmethod
+    def forward(ctx, x):
+        x = x.contiguous()
+        B, T, Cc = x.shape
+        y = torch.empty((B, Cc), dtype=x.dtype, device=x.device)
+        K.time_mean_fwd(x, y)
+        ctx.shape = x.shape
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        dx = torch.empty(ctx.shape, dtype=dy.dtype, device=dy.device)
+        K.time_mean_bwd(dy.contiguous(), dx)
+        return dx
+
+
+def time_mean(x):
+    return TimeMeanFn.apply(x)

@@ -121,6 +121,14 @@ class SpeechT5Task(LegacyFairseqTask):
             encoder_input.update(kwargs)
             return models[0].generate_speech(**encoder_input)
 
+    def generate_class(self, models, net_input, prefix_tokens, **kwargs):
+        """tasks/speecht5.py:631-638 (what scripts/generate_class.py calls): the predicted class of every utterance."""
+        with torch.no_grad():
+            encoder_input = {k: v for k, v in net_input.items() if k not in ("prev_output_tokens", "task_name")}
+            encoder_input.update(kwargs)
+            encoder_input.update({"prev_output_tokens": prefix_tokens})
+            return models[0].generate_class(**encoder_input)
+
     def build_model(self, args):
         args.speech_odim = 80  # tasks/speecht5.py:581-597
         return T5TransformerModel.build_model(args, self)

@@ -477,7 +477,7 @@ class B200Trainer:
         here -- same stream, same order -- and hands them to forward() as explicit inputs."""
         prenet = getattr(self.model, "speech_encoder_prenet", None)
         ni = sample.get("net_input", {})
-        if (sample.get("task_name") != "s2t" or prenet is None or not self.model.training or "mask_indices" in ni
+        if (sample.get("task_name") not in ("s2t", "s2c") or prenet is None or not self.model.training or "mask_indices" in ni
                 or (prenet.mask_prob <= 0 and getattr(prenet, "mask_channel_prob", 0.0) <= 0)):
             return sample
         from .data import draw_hubert_masks
