@@ -1,9 +1,11 @@
 // Batched bf16 GEMM on the Hopper tensor cores (wgmma, fp32 accumulators in registers), operands staged by TMA into
 // 128B-swizzled shared memory through an mbarrier ring. One CTA computes a 128 x BN output tile.
 //
-// Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread), warpgroups 1..2 = consumers: each issues
-// the wgmma of 64 rows of the tile, then all 8 consumer warps run the epilogue (accumulators -> swizzled shared
-// memory -> one row x 32 columns per thread -> fused bias / activation / dropout / residual -> global).
+// Warp roles (512 threads): warpgroup 0 = TMA producer (one elected thread), warpgroups 1..2 = MMA: each issues the
+// wgmma of 64 rows of the tile and hands the accumulators over through a swizzled fp32 tile in shared memory,
+// warpgroup 3 = epilogue (one row x 32 columns per thread -> fused bias / activation / dropout / residual -> global).
+// The handoff is a pair of mbarriers, so the MMA warpgroups start the next tile's main loop while the epilogue drains
+// this one; on a CTA's last tile they have nothing left to multiply and join the epilogue (12 warps).
 //
 // This one kernel is the contraction engine for every dense op on the SpeechT5 path: the q/k/v/out projections
 // (reference: speecht5/models/modules/multihead_attention.py:213-231,397), the FFN (transformer_layer.py:127-132,
@@ -24,8 +26,13 @@ namespace st5 {
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 bytes = one swizzle row
 constexpr int MMA_K = 16;
-constexpr int EPI_WARPS = 8;  // the consumer warps: 4 row quarters x 2 column groups, each taking every 2nd 32-column chunk
-constexpr int GEMM_THREADS = 128 + 32 * EPI_WARPS;
+constexpr int MMA_WARPS = 8;  // two warpgroups, rows [0, 64) and [64, 128) of the tile
+constexpr int EPI_WARPS = 4;  // one warpgroup: warp w takes row quarter w and every 32-column chunk
+constexpr int GEMM_THREADS = 128 + 32 * (MMA_WARPS + EPI_WARPS);
+// Registers per thread after setmaxnreg (producer / MMA / epilogue warpgroup): 40 + 2 * 160 + 152 = 4 * 128, the file
+// of one 512-thread CTA.
+constexpr int REGS_PRODUCER = 40, REGS_MMA = 160, REGS_EPI = 152;
+static_assert(REGS_PRODUCER + 2 * REGS_MMA + REGS_EPI <= 65536 / 128, "register plan exceeds the register file");
 
 struct EpiParams {
   int M, N, nb1;
@@ -109,119 +116,26 @@ __device__ __forceinline__ void gemm_mainloop(float (&acc)[BN / 2], const uint8_
   if (leader) mbar_arrive(&empty_bar[prev]);
 }
 
-// fp32 accumulator tile in shared memory, [BLOCK_M][BN] with the 16-byte column groups of row r XOR-ed by r % 8:
-// the epilogue's row-per-lane float4 reads are conflict-free.
-template <int BN>
+// fp32 accumulator tile in shared memory, chunk-major [BN / 32][BLOCK_M][32], the 16-byte column groups of row r XOR-ed
+// by r % 8: the epilogue's row-per-lane float4 reads are conflict-free, and the 32 x 32 block of one row quarter and
+// one 32-column chunk is 4 KB of contiguous, 1 KB-aligned memory. That block is the staging buffer of the warp that
+// finishes it: the fp32 TMA store box (128B swizzle) has exactly this layout, a bf16 one (64B swizzle) fits in either
+// 2 KB half, so two bf16 outputs of one chunk (C_pre and C, or the gate epilogue's pair) take one half each.
 __device__ __forceinline__ int acc_idx(int row, int col) {
-  return row * BN + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3));
+  return (col >> 5) * (BLOCK_M * 32) + row * 32 + (((((col >> 2) ^ row) & 7) << 2) | (col & 3));
 }
 
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(32 * EPI_WARPS) : "memory"); }
-
-template <int BN, int STAGES, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_wgmma(const __grid_constant__ CUtensorMap map_a,
-                                                                const __grid_constant__ CUtensorMap map_b,
-                                                                const __grid_constant__ CUtensorMap map_c,
-                                                                const __grid_constant__ CUtensorMap map_cpre,
-                                                                const EpiParams p) {
-  constexpr uint32_t A_BYTES = BLOCK_M * BLOCK_K * 2;
-  constexpr uint32_t B_BYTES = BN * BLOCK_K * 2;
-  constexpr uint32_t CHUNK_BYTES = 64 * BLOCK_K * 2;  // one 64(mn) x 64(k) MN-major box
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * A_BYTES;
-  float* sacc = reinterpret_cast<float*>(smem_b + STAGES * B_BYTES);        // BLOCK_M x BN fp32 accumulators
-  uint8_t* stg_all = reinterpret_cast<uint8_t*>(sacc + BLOCK_M * BN);        // EPI_WARPS x 4 KB TMA-store staging
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_all + EPI_WARPS * 4096);
-  uint64_t* empty_bar = full_bar + STAGES;
-
-  // Persistent CTA: loops over output tiles (m fastest, so concurrently running CTAs share the B/weight tile in L2);
-  // the producer runs ahead into the next tile while the consumers drain the current one.
-  const int warp = threadIdx.x >> 5;
-  const int nkb = p.num_k_blocks;
-  const int tiles_mn = p.tiles_m * p.tiles_n;
-
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&map_a);
-    tma_prefetch_desc(&map_b);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  // Programmatic dependent launch: everything above touched only this CTA's shared memory, so it may run while the
-  // preceding grid drains. Wait for that grid's memory here, before the first global access, and let the grid behind
-  // us start its own prologue (both are no-ops when the launch carries no programmatic attribute).
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-
-  if (warp < 4) {
-    // ===================== TMA producer =====================
-    setmaxnreg_dec<40>();
-    if (warp == 0 && elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int z = tile / tiles_mn, rmn = tile - z * tiles_mn;
-      const int m0 = (rmn % p.tiles_m) * BLOCK_M, n0 = (rmn / p.tiles_m) * BN;
-      const int b1 = z % p.nb1, b2 = z / p.nb1;
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait_quiet(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem_a + stage * A_BYTES;
-        uint8_t* sb = smem_b + stage * B_BYTES;
-        const int k0 = kb * BLOCK_K;
-        mbar_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
-        if (A_MN) {
-#pragma unroll
-          for (int c = 0; c < BLOCK_M / 64; ++c)
-            tma_load_4d(sa + c * CHUNK_BYTES, &map_a, &full_bar[stage], m0 + c * 64, k0, b1 * p.a_m1, b2 * p.a_m2);
-        } else {
-          tma_load_4d(sa, &map_a, &full_bar[stage], k0, m0, b1 * p.a_m1, b2 * p.a_m2);
-        }
-        if (B_MN) {
-#pragma unroll
-          for (int c = 0; c < BN / 64; ++c)
-            tma_load_4d(sb + c * CHUNK_BYTES, &map_b, &full_bar[stage], n0 + c * 64, k0, b1 * p.b_m1, b2 * p.b_m2);
-        } else {
-          tma_load_4d(sb, &map_b, &full_bar[stage], k0, n0, b1 * p.b_m1, b2 * p.b_m2);
-        }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      }
-    }
-  } else {
-    // ===================== consumers: wgmma main loop, then the epilogue =====================
-    setmaxnreg_inc<232>();
-    const int cw = warp - 4;                     // consumer warp 0..7
-    const int wg = cw >> 2;                      // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
-    const int q = cw & 3;                        // epilogue: row quarter [32 q, 32 q + 32)
-    constexpr int NGRP = EPI_WARPS / 4;
-    const int grp = cw >> 2;                     // epilogue: 32-column chunks c = grp, grp + NGRP, ...
-    uint8_t* stg = stg_all + cw * 4096;
-    uint64_t dseed = p.drop_seed, doffset = p.drop_offset;
-    if (p.drop_thr != 0) resolve_seed(dseed, doffset);
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+// The fused epilogue of one output tile for one warp: rows [32 q, 32 q + 32) of the tile (one per lane), 32-column
+// chunks c = grp, grp + ngrp, ... Every output block leaves by TMA from its own 32 x 32 block of `sacc`; the caller
+// waits for those bulk stores to have read shared memory before the tile's accumulators may be overwritten.
+template <int BN>
+__device__ __forceinline__ void epilogue_tile(const EpiParams& p, float* sacc, const CUtensorMap& map_c,
+                                              const CUtensorMap& map_cpre, int tile, int q, int grp, int ngrp,
+                                              uint64_t dseed, uint64_t doffset) {
+    const int tiles_mn = p.tiles_m * p.tiles_n;
     const int z = tile / tiles_mn, rmn = tile - z * tiles_mn;
     const int m0 = (rmn % p.tiles_m) * BLOCK_M, n0 = (rmn / p.tiles_m) * BN;
     const int b1 = z % p.nb1, b2 = z / p.nb1;
-    {
-      float acc[BN / 2];
-      gemm_mainloop<BN, A_MN, B_MN>(acc, smem_a, smem_b, full_bar, empty_bar, stage, phase, nkb, wg, STAGES);
-      consumer_sync();  // the previous tile's epilogue has read the accumulator tile
-      const int l = (int)lane_id();
-      const int rbase = wg * 64 + (cw & 3) * 16 + (l >> 2);
-#pragma unroll
-      for (int i = 0; i < BN / 2; i += 2) {
-        const int rr = rbase + 8 * ((i >> 1) & 1), cc = 8 * (i >> 2) + 2 * (l & 3);
-        *reinterpret_cast<float2*>(sacc + acc_idx<BN>(rr, cc)) = make_float2(acc[i], acc[i + 1]);
-      }
-      consumer_sync();
-    }
     const int row = m0 + q * 32 + (int)lane_id();
     const bool row_ok = row < p.M;
     const long zoff = (long)b1 * p.c_bs1 + (long)b2 * p.c_bs2;
@@ -229,15 +143,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_wgmma(const __grid_
     const float* bias2_row = (p.bias2 != nullptr && row_ok) ? p.bias2 + (long)(row / p.bias2_rows) * p.N : nullptr;
     const uint64_t drop_row = ((uint64_t)z * (uint64_t)p.M + (uint64_t)row) * (uint64_t)p.N;
 #pragma unroll 1
-    for (int c = grp; c < BN / 32; c += NGRP) {
+    for (int c = grp; c < BN / 32; c += ngrp) {
       const int nb = n0 + c * 32;
       if (nb >= p.N) continue;  // warp-uniform; rows beyond M keep going (their loads are guarded, stores clipped)
+      uint8_t* const blk = reinterpret_cast<uint8_t*>(sacc + acc_idx(q * 32, c * 32));  // this warp's 32 x 32 block
+      bool staged = false;  // a bulk store of this chunk is reading the block
       float v[32];
       {
         const int tr = q * 32 + (int)lane_id();
 #pragma unroll
         for (int j = 0; j < 32; j += 4) {
-          const float4 a4 = *reinterpret_cast<const float4*>(sacc + acc_idx<BN>(tr, c * 32 + j));
+          const float4 a4 = *reinterpret_cast<const float4*>(sacc + acc_idx(tr, c * 32 + j));
           v[j] = a4.x; v[j + 1] = a4.y; v[j + 2] = a4.z; v[j + 3] = a4.w;
         }
       }
@@ -288,8 +204,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_wgmma(const __grid_
       // clipped at the tensor edges); fall back to per-thread stores when the output layout is not TMA-addressable.
       auto emit = [&](void* base, const CUtensorMap* tmap) {
         if (p.tma_store) {
-          if (lane_id() == 0) bulk_wait_read0();  // previous block of this warp has left the staging buffer
-          __syncwarp();
+          // The second output of a chunk (C after C_pre): bf16 takes the free second half of the block, fp32 waits
+          // until the C_pre store has read the block.
+          uint8_t* const stg = staged && !p.c_fp32 ? blk + 2048 : blk;
+          if (staged && p.c_fp32 && lane_id() == 0) bulk_wait_read0();
+          __syncwarp();  // (also: every lane has read its accumulators out of the block)
+          staged = true;
           const int rr = (int)lane_id();
           if (p.c_fp32) {
 #pragma unroll
@@ -357,8 +277,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_wgmma(const __grid_
         // both). The dH = dO.W2 GEMM of the backward then multiplies by it -- no Philox, no tanh in that epilogue.
         // Eight columns at a time straight into the two halves of this warp's staging block (bf16: 2 KB each), so
         // the chunk is never held twice in registers. Launcher guarantees: bf16 output, TMA-store layout, N % 8 == 0.
-        if (lane_id() == 0) bulk_wait_read0();
-        __syncwarp();
+        __syncwarp();  // every lane has read its accumulators out of the block
         const int rr = (int)lane_id();
         const uint64_t e0 = drop_row + (uint64_t)nb;
 #pragma unroll
@@ -396,14 +315,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_wgmma(const __grid_
             pd.z = *reinterpret_cast<uint32_t*>(&u2); pd.w = *reinterpret_cast<uint32_t*>(&u3);
           }
           const int so = rr * 64 + ((g ^ ((rr >> 1) & 3)) << 4);
-          *reinterpret_cast<uint4*>(stg + so) = po;
-          *reinterpret_cast<uint4*>(stg + 2048 + so) = pd;
+          *reinterpret_cast<uint4*>(blk + so) = po;
+          *reinterpret_cast<uint4*>(blk + 2048 + so) = pd;
         }
         fence_proxy_async();
         __syncwarp();
         if (lane_id() == 0) {
-          tma_store_4d(&map_c, stg, nb, m0 + q * 32, b1, b2);
-          tma_store_4d(&map_cpre, stg + 2048, nb, m0 + q * 32, b1, b2);
+          tma_store_4d(&map_c, blk, nb, m0 + q * 32, b1, b2);
+          tma_store_4d(&map_cpre, blk + 2048, nb, m0 + q * 32, b1, b2);
           bulk_commit();
         }
         continue;
@@ -479,8 +398,134 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_wgmma(const __grid_
       }
       emit(p.C, &map_c);
     }
+}
+
+template <int BN, int STAGES, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_wgmma(const __grid_constant__ CUtensorMap map_a,
+                                                                const __grid_constant__ CUtensorMap map_b,
+                                                                const __grid_constant__ CUtensorMap map_c,
+                                                                const __grid_constant__ CUtensorMap map_cpre,
+                                                                const __grid_constant__ EpiParams p) {
+  constexpr uint32_t A_BYTES = BLOCK_M * BLOCK_K * 2;
+  constexpr uint32_t B_BYTES = BN * BLOCK_K * 2;
+  constexpr uint32_t CHUNK_BYTES = 64 * BLOCK_K * 2;  // one 64(mn) x 64(k) MN-major box
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + STAGES * A_BYTES;
+  float* sacc = reinterpret_cast<float*>(smem_b + STAGES * B_BYTES);  // BLOCK_M x BN fp32 accumulators
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sacc + BLOCK_M * BN);
+  uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* sacc_full = empty_bar + STAGES;  // a tile's accumulators are in sacc (one arrive per MMA warp)
+  uint64_t* sacc_empty = sacc_full + 1;      // the epilogue is done with them (one arrive per epilogue warp)
+
+  // Persistent CTA: loops over output tiles (m fastest, so concurrently running CTAs share the B/weight tile in L2);
+  // the producer runs ahead into the next tile, and the MMA warps start it while the epilogue drains this one. Every
+  // role walks the same tile sequence; the i-th tile of a CTA is the i-th phase of sacc_full and sacc_empty.
+  const int warp = threadIdx.x >> 5;
+  const int nkb = p.num_k_blocks;
+  const int tiles_mn = p.tiles_m * p.tiles_n;
+
+  if (warp == 0 && elect_one()) {
+    tma_prefetch_desc(&map_a);
+    tma_prefetch_desc(&map_b);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);  // one arrive per MMA warpgroup
     }
-    if (p.tma_store && lane_id() == 0) bulk_wait_read0();  // staging buffer must outlive the last bulk store
+    mbar_init(sacc_full, MMA_WARPS);
+    mbar_init(sacc_empty, EPI_WARPS);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  // Programmatic dependent launch: everything above touched only this CTA's shared memory, so it may run while the
+  // preceding grid drains. Wait for that grid's memory here, before the first global access, and let the grid behind
+  // us start its own prologue (both are no-ops when the launch carries no programmatic attribute).
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+  if (warp < 4) {
+    // ===================== TMA producer =====================
+    setmaxnreg_dec<REGS_PRODUCER>();
+    if (warp == 0 && elect_one()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      const int z = tile / tiles_mn, rmn = tile - z * tiles_mn;
+      const int m0 = (rmn % p.tiles_m) * BLOCK_M, n0 = (rmn / p.tiles_m) * BN;
+      const int b1 = z % p.nb1, b2 = z / p.nb1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait_quiet(&empty_bar[stage], phase ^ 1);
+        uint8_t* sa = smem_a + stage * A_BYTES;
+        uint8_t* sb = smem_b + stage * B_BYTES;
+        const int k0 = kb * BLOCK_K;
+        mbar_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
+        if (A_MN) {
+#pragma unroll
+          for (int c = 0; c < BLOCK_M / 64; ++c)
+            tma_load_4d(sa + c * CHUNK_BYTES, &map_a, &full_bar[stage], m0 + c * 64, k0, b1 * p.a_m1, b2 * p.a_m2);
+        } else {
+          tma_load_4d(sa, &map_a, &full_bar[stage], k0, m0, b1 * p.a_m1, b2 * p.a_m2);
+        }
+        if (B_MN) {
+#pragma unroll
+          for (int c = 0; c < BN / 64; ++c)
+            tma_load_4d(sb + c * CHUNK_BYTES, &map_b, &full_bar[stage], n0 + c * 64, k0, b1 * p.b_m1, b2 * p.b_m2);
+        } else {
+          tma_load_4d(sb, &map_b, &full_bar[stage], k0, n0, b1 * p.b_m1, b2 * p.b_m2);
+        }
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      }
+    }
+  } else if (warp < 4 + MMA_WARPS) {
+    // ===================== MMA: wgmma main loop, accumulators -> sacc =====================
+    setmaxnreg_inc<REGS_MMA>();
+    const int mw = warp - 4;  // MMA warp 0..7
+    const int wg = mw >> 2;   // MMA warpgroup: rows [64 wg, 64 wg + 64) of the tile
+    const int ntiles = (p.num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // >= 1: grid <= tiles
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int it = 0; it < ntiles; ++it) {
+      float acc[BN / 2];
+      gemm_mainloop<BN, A_MN, B_MN>(acc, smem_a, smem_b, full_bar, empty_bar, stage, phase, nkb, wg, STAGES);
+      mbar_wait_quiet(sacc_empty, (it & 1) ^ 1);  // the epilogue of the previous tile is done with sacc
+      // acc[i], acc[i + 1] -> acc_idx(row, col), row = 16 w + l / 4 + 8 ((i >> 1) & 1), col = 8 (i >> 2) + 2 (l % 4),
+      // spelled as one lane base plus compile-time offsets (the 16-byte group (col / 4) % 8 = (2 (i >> 2)) % 8 ^ (l / 2)
+      // % 2, XOR-ed by row % 8 = (l / 4) % 8): few live registers across the main loop.
+      const int l = (int)lane_id();
+      const int sw = ((l >> 1) & 1) ^ ((l >> 2) & 7);
+      float* const abase = sacc + (wg * 64 + (mw & 3) * 16 + (l >> 2)) * 32 + 2 * (l & 1);
+#pragma unroll
+      for (int i = 0; i < BN / 2; i += 2)
+        *reinterpret_cast<float2*>(abase + (i >> 4) * (BLOCK_M * 32) + 256 * ((i >> 1) & 1) +
+                                   ((((2 * (i >> 2)) & 7) ^ sw) << 2)) = make_float2(acc[i], acc[i + 1]);
+      __syncwarp();
+      if (l == 0) mbar_arrive(sacc_full);
+    }
+    // The CTA's last tile: nothing left to multiply, so these 8 warps join the epilogue warpgroup -- 12 warps, 4 row
+    // quarters x 3 column groups (a CTA with a single tile, e.g. a split-K weight gradient, would otherwise drain it on
+    // 4 warps). Outside the tile loop, so that the epilogue's registers do not compete with the main loop's.
+    uint64_t dseed = p.drop_seed, doffset = p.drop_offset;
+    if (p.drop_thr != 0) resolve_seed(dseed, doffset);
+    mbar_wait_quiet(sacc_full, (ntiles - 1) & 1);
+    epilogue_tile<BN>(p, sacc, map_c, map_cpre, (int)blockIdx.x + (ntiles - 1) * (int)gridDim.x, mw & 3, mw >> 2, 3,
+                      dseed, doffset);
+    if (lane_id() == 0) bulk_wait_read0();  // sacc must outlive the last bulk store
+  } else {
+    // ===================== epilogue: sacc -> fused epilogue -> global =====================
+    setmaxnreg_inc<REGS_EPI>();
+    const int ew = warp - 4 - MMA_WARPS;  // row quarter of this warp
+    uint64_t dseed = p.drop_seed, doffset = p.drop_offset;
+    if (p.drop_thr != 0) resolve_seed(dseed, doffset);
+    for (int tile = blockIdx.x, it = 0; tile < p.num_tiles; tile += gridDim.x, ++it) {
+      mbar_wait_quiet(sacc_full, it & 1);
+      const bool last = tile + (int)gridDim.x >= p.num_tiles;  // then the MMA warps take column groups 0 and 1
+      epilogue_tile<BN>(p, sacc, map_c, map_cpre, tile, ew, last ? 2 : 0, last ? 3 : 1, dseed, doffset);
+      if (lane_id() == 0) bulk_wait_read0();  // this warp's bulk stores have read their staging out of sacc
+      __syncwarp();
+      if (!last && lane_id() == 0) mbar_arrive(sacc_empty);
+    }
   }
 }
 
@@ -586,7 +631,7 @@ static int launch_variant(const GemmDesc& g, const EpiParams& ep, cudaStream_t s
   rc = make_operand_map(&mb, g.B, g.b_mn, g.N, g.K, g.b_ld, g.nb1, g.b_bs1, g.nb2, g.b_bs2, BN);
   if (rc) return rc - 10;
   constexpr size_t smem = (size_t)STAGES * (BLOCK_M * BLOCK_K * 2 + BN * BLOCK_K * 2) + BLOCK_M * BN * 4 +
-                          EPI_WARPS * 4096 + 2 * STAGES * 8 + 1024;
+                          (2 * STAGES + 2) * 8 + 1024;
   static_assert(smem <= 227 * 1024, "GEMM tile does not fit the 227 KB of shared memory of a block");
   auto kern = gemm_bf16_wgmma<BN, STAGES, A_MN, B_MN>;
   static bool attr_set = false;
