@@ -180,6 +180,9 @@ class TexttoSpeechLoss(FairseqCriterion):
             raise ValueError("unknown --loss-type " + self.loss_type)
         enc_dec_attn_loss = None
         if self.use_guided_attn_loss and "encoder-decoder" in self.modules_applied_guided_attn:
+            if sample.get("task_name") == "s2s" and getattr(model, "speech_encoder_prenet", None) is not None:
+                # (:198-206) a waveform source: the encoder sees the conv front end's frames, not the samples
+                ilens = model.speech_encoder_prenet.get_src_lengths(ilens)
             attn = list(attn) if isinstance(attn, (list, tuple)) else [attn]
             if fused:
                 enc_dec_attn_loss = GuidedAttnFn.apply(ilens, sample["dec_target_lengths"], r,

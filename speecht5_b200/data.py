@@ -204,6 +204,55 @@ def synthetic_sid_batch(B, n_samples, n_classes, seed=1, ragged=True, pin=False)
     return _pin(sample) if pin else sample
 
 
+def collate_vc(samples, reduction_factor=2):
+    """SpeechToSpeechDataset.collater (speecht5/data/speech_to_speech_dataset.py:169-228) over in-memory items
+    {"id", "source": FloatTensor [N] waveform, "target": FloatTensor [L, odim] log-mel, "spkembs": FloatTensor [512],
+    "audio_name", "tgt_name"}: zero-padded waveforms with their padding mask, the target frames padded, the decoder input
+    = a zero frame then every r-th target frame ([r-1::r], last one dropped), stop labels 1 from the last real frame on,
+    src_lengths / ntokens in waveform samples. Host-side work only."""
+    samples = [s for s in samples if s["source"] is not None]
+    if len(samples) == 0:
+        return {}
+    audio_sizes = [len(s["source"]) for s in samples]
+    source, padding_mask = _collate_audio([s["source"] for s in samples])
+    fbank_sizes = [len(s["target"]) for s in samples]
+    fbanks = collate_frames([s["target"] for s in samples])
+    sizes = torch.tensor(fbank_sizes, dtype=torch.long)
+    r = reduction_factor
+    if r > 1:
+        fb_in, sizes_in = fbanks[:, r - 1::r], torch.div(sizes, r, rounding_mode="floor")
+    else:
+        fb_in, sizes_in = fbanks, sizes
+    prev = torch.cat([fb_in.new_zeros((fb_in.shape[0], 1, fb_in.shape[2])), fb_in[:, :-1]], dim=1)
+    labels = fbanks.new_zeros(fbanks.size(0), fbanks.size(1))
+    for i, n in enumerate(fbank_sizes):
+        labels[i, n - 1:] = 1.0
+    spkembs = collate_frames([s["spkembs"] for s in samples], is_audio_input=True)
+    net_input = {"source": source, "padding_mask": padding_mask, "prev_output_tokens": prev, "tgt_lengths": sizes_in,
+                 "spkembs": spkembs, "task_name": "s2s"}
+    return {"id": torch.LongTensor([s["id"] for s in samples]), "name": [s.get("audio_name") for s in samples],
+            "tgt_name": [s.get("tgt_name") for s in samples], "net_input": net_input, "labels": labels,
+            "dec_target": fbanks, "dec_target_lengths": sizes, "src_lengths": torch.LongTensor(audio_sizes),
+            "task_name": "s2s", "ntokens": sum(audio_sizes), "target": fbanks}
+
+
+def synthetic_vc_batch(B, n_samples, T_mel, seed=1, ragged=True, pin=False, odim=80, reduction_factor=2):
+    """Voice-conversion batch through the s2s collater: source waveforms N(0, 0.1^2) with lengths U{0.8 n .. n},
+    target log-mels N(0, 1) [L, odim] with L U{0.8 T .. T} (the first utterance n samples / T frames), 512-d
+    x-vectors."""
+    g = torch.Generator().manual_seed(seed)
+    items = []
+    for b in range(B):
+        n, L = n_samples, T_mel
+        if ragged and b > 0:
+            n = int(torch.randint(int(0.8 * n_samples), n_samples + 1, (1,), generator=g))
+            L = int(torch.randint(int(0.8 * T_mel), T_mel + 1, (1,), generator=g))
+        items.append({"id": b, "source": torch.randn(n, generator=g) * 0.1,
+                      "target": torch.randn(L, odim, generator=g), "spkembs": torch.randn(512, generator=g)})
+    sample = collate_vc(items, reduction_factor)
+    return _pin(sample) if pin else sample
+
+
 def _span_lengths(rng, kind, count, length, other):
     """Span lengths of one row; each non-static kind consumes `count` draws from the stream, like the reference."""
     if kind == "static":

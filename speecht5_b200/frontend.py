@@ -445,6 +445,10 @@ class SpeechEncoderPrenet(torch.nn.Module):
     def set_num_updates(self, num_updates):
         self.num_updates = num_updates
 
+    def get_src_lengths(self, src_lengths):
+        """speech_encoder_prenet.py:231-232: frames the conv front end makes of waveforms of these sample counts."""
+        return self.feature_extractor.get_out_seq_lens_tensor(src_lengths)
+
     def forward(self, src_tokens, require_feat_pen=False, target_list=None, padding_mask=None, mask=True,
                 mask_indices=None, mask_channel_indices=None):
         """Reference signature and returns (speech_encoder_prenet.py:151-204): `(x, frame_padding_mask)`, or with

@@ -31,6 +31,19 @@ def _fold_residual_grad(x):
     return torch.is_grad_enabled() and x.requires_grad and ops.RT.fold_residual_grad
 
 
+def _keep_or_skip(keep, y, x):
+    """LayerDrop under CUDA-graph capture: the layer's output where `keep` (device 0/1 flag) is set, else its input --
+    together with the fp32 copy of the residual stream (ops.residual_layer_norm), so that the next layer adds the same
+    residual an eager update that ran or skipped this layer would. A side without a copy (the stack's input) is a bf16
+    tensor whose fp32 value is exact."""
+    on = keep > 0.5
+    out = torch.where(on, y, x)
+    y32, x32 = getattr(y, "_st5_f32", None), getattr(x, "_st5_f32", None)
+    if y32 is not None or x32 is not None:
+        out._st5_f32 = torch.where(on, y32 if y32 is not None else y.float(), x32 if x32 is not None else x.float())
+    return out
+
+
 class MultiheadAttention(nn.Module):
     """Parameter holder with the reference's names (q/k/v/out_proj Linear); compute happens in the owning layer through
     ops.linear (fused q|k|v projection) + ops.attention."""
@@ -223,15 +236,18 @@ class TransformerEncoder(nn.Module):
                 pos_k, maxpos = self.pos_emb.pe_k.weight, self.pos_emb.maxlen
         r = d = None
         keep_dev, keep_host = RT.layer_keep, RT.layer_keep_host
+        blocks, base = self.training and (keep_dev is not None or keep_host is not None), RT._offset
         for i, layer in enumerate(self.layers):
             x = RT.stage(("enc", i), x)  # gradient-exchange overlap point (trainer), identity otherwise
+            if blocks:
+                RT.offset_block(base, i)
             frozen = (not ft) and i not in self.no_freeze_encoder_layer
             with torch.no_grad() if frozen else contextlib.ExitStack():
                 if self.training and keep_dev is not None:
                     # LayerDrop under CUDA-graph capture: the trainer drew the subset (same numpy stream as :252); a
                     # dropped layer's output is replaced by its input, its parameters receive exactly zero gradient
                     y, _ = layer(x, self_attn_padding_mask=encoder_padding_mask, pos_bias=pos_k, maxpos=maxpos)
-                    x = torch.where(keep_dev[i] > 0.5, y, x)
+                    x = _keep_or_skip(keep_dev[i], y, x)
                 else:
                     if keep_host is not None:
                         run = bool(keep_host[i] > 0.5)
@@ -247,6 +263,8 @@ class TransformerEncoder(nn.Module):
                     break
                 if return_all_hiddens:
                     encoder_states.append(x.transpose(0, 1))
+        if blocks:
+            RT.offset_block(base, len(self.layers))
         with torch.no_grad() if not ft else contextlib.ExitStack():
             if self.layer_norm_first:
                 x = ops.residual_layer_norm(x, None, self.layer_norm)
@@ -413,13 +431,16 @@ class TransformerDecoder(nn.Module):
         keep_dev, keep_host = RT.layer_keep, RT.layer_keep_host
         n_enc = 0 if (keep_dev is None and keep_host is None) else (len(keep_dev if keep_dev is not None else keep_host)
                                                                     - len(self.layers))
+        blocks, base = self.training and (keep_dev is not None or keep_host is not None), RT._offset
         for idx, layer in enumerate(self.layers):
             x = RT.stage(("dec", idx), x)  # gradient-exchange overlap point (trainer), identity otherwise
+            if blocks:
+                RT.offset_block(base, idx)
             want = bool(idx == alignment_layer or alignment_layer == -1)
             if self.training and keep_dev is not None:  # LayerDrop under capture: see TransformerEncoder
                 y, layer_attn, _ = layer(x, enc, padding_mask, causal=not full_context_alignment,
                                          self_attn_padding_mask=tgt_mask, need_attn=want, need_head_weights=want)
-                x = torch.where(keep_dev[n_enc + idx] > 0.5, y, x)
+                x = _keep_or_skip(keep_dev[n_enc + idx], y, x)
                 # (the reference drops the layer's attention map from the list too; under a static graph it stays, the
                 #  s2t / pre-training criteria that use LayerDrop do not read it)
             else:
@@ -435,6 +456,8 @@ class TransformerDecoder(nn.Module):
             if layer_attn is not None and want:
                 attn = layer_attn.float()
                 attn_list.append(attn)  # [B,H,T,S] == reference attn.transpose(0, 1)
+        if blocks:
+            RT.offset_block(base, len(self.layers))
         if attn is not None and len(attn_list) == 1:
             if alignment_heads is not None:
                 attn = attn[:, :alignment_heads]

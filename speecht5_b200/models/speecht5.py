@@ -6,9 +6,10 @@ t5_transformer_base, t5_transformer_large, t5_transformer_base_asr :1252,1385,14
 Coverage of forward(): text -> speech (t2s, the BASELINE.json metric path), speech -> text (s2t: waveform front end,
 CE + CTC), text -> text (t2t / text pre-training), speech pre-training (HuBERT targets, masked-prediction head, shared
 Gumbel quantizer, reconstruction through the speech decoder; only_hubert / feature_only returns), speaker
-identification (s2c: speaker head on the pooled decoder or encoder state, margin softmax), greedy generation of speech
-and text, class prediction. The branches SURVEY.md section 2 leaves out (voice conversion / enhancement s2s inputs)
-raise NotImplementedError rather than silently falling back to PyTorch."""
+identification (s2c: speaker head on the pooled decoder or encoder state, margin softmax), voice conversion (s2s:
+waveform in, log-mel out, x-vector in the decoder prenet), greedy generation of speech (from text or from speech) and
+text, class prediction. The branches left out (the speech-enhancement s2s variants) raise NotImplementedError rather
+than silently falling back to PyTorch."""
 import argparse
 import logging
 from argparse import Namespace
@@ -263,6 +264,8 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
                 logit_temp=getattr(args, "logit_temp", 0.1), untie_final_proj=getattr(args, "untie_final_proj", True),
                 skip_masked=getattr(args, "skip_masked", False), skip_nomask=getattr(args, "skip_nomask", False),
                 target_glu=getattr(args, "target_glu", False))
+        if getattr(task, "t5_task", None) == "s2s":
+            _check_vc_options(args)
         # speaker-identification head (:709-715): one class per entry of the task's text dictionary
         speaker_decoder_postnet = None
         if getattr(task, "t5_task", None) == "s2c":
@@ -295,7 +298,7 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
         if not built:
             raise NotImplementedError(
                 f"T5TransformerModel.forward: {input_type}->{output_type} (task {task_name}) is not built in the H100 "
-                "path (speaker identification / voice conversion / enhancement branches)")
+                "path (speech input needs --build-speech-encoder, text output --build-text-decoder)")
         features_pen = frame_mask_indices = None
         if speech_in and target_list is not None:  # (:813-815) speech pre-training: frames aligned with the labels
             enc_in, encoder_padding_mask = self.speech_encoder_prenet(
@@ -554,10 +557,12 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
 
     @torch.no_grad()
     def generate_speech(self, source=None, src_tokens=None, spkembs=None, **kwargs):
-        """models/speecht5.py:1188-1249, text input: greedy frame-by-frame synthesis until a stop probability of the
-        current r-frame group reaches the threshold (or maxlen). Same knobs and quirk as the reference, which reads
-        kwargs["threshold"] for the threshold, minlenratio AND maxlenratio (:1190-1199); defaults 0.5 / 0.0 / 20.0.
-        Returns (mel [L, odim] fp32, stop probabilities [L], cross-attention [layers, H, L/r, T_text]).
+        """models/speecht5.py:1188-1249: greedy frame-by-frame synthesis until a stop probability of the current r-frame
+        group reaches the threshold (or maxlen), from text tokens (TTS) or from a waveform `source` with its
+        `padding_mask` (voice conversion; the encoder runs on the waveform's conv frames). Same knobs and quirk as the
+        reference, which reads kwargs["threshold"] for the threshold, minlenratio AND maxlenratio (:1190-1201); defaults
+        0.5 / 0.0 / 20.0 for text, 0.5 / 0.0 / 10.0 for speech. Batch size 1 (asserted, as in the reference).
+        Returns (mel [L, odim] fp32, stop probabilities [L], cross-attention [layers, H, L/r, T_enc]).
 
         use_cache=False re-runs the decoder on the whole prefix every step (causal self-attention makes that equal to
         the reference's incremental state, and every step reuses the training kernels; the always-on prenet dropout then
@@ -565,20 +570,24 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
         -- identical in distribution for the newest frame); use_cache=True keeps a key/value cache, "graph" replays one
         captured CUDA graph per decoder step (speecht5_b200/incremental.py)."""
         assert source is not None or src_tokens is not None
-        if source is not None:
-            raise NotImplementedError("generate_speech from speech input (voice conversion, out of scope: SURVEY.md section 2)")
-        assert src_tokens.size(0) == 1
         threshold = kwargs.get("threshold", 0.5)
         minlenratio = kwargs.get("threshold", 0.0)
-        maxlenratio = kwargs.get("threshold", 20.0)
         if spkembs is not None and getattr(self.args, "spk_embed_integration_type", "pre") != "pre":
             raise NotImplementedError("spk_embed_integration_type != 'pre'")
-        encoder_out = self.forward_text_encoder(src_tokens)
+        if source is None:
+            assert src_tokens.size(0) == 1
+            encoder_out = self.forward_text_encoder(src_tokens)
+            maxlenratio = kwargs.get("threshold", 20.0)
+        else:
+            assert source.size(0) == 1
+            encoder_out = self.forward_encoder(source, padding_mask=kwargs.get("padding_mask"))
+            maxlenratio = kwargs.get("threshold", 10.0)
+        dev = (source if source is not None else src_tokens).device
         post = self.speech_decoder_postnet
         r, odim = self.reduction_factor, post.odim
         T_enc = encoder_out["encoder_out"][0].size(0)
         maxlen, minlen = int(T_enc * maxlenratio / r), int(T_enc * minlenratio / r)
-        ys = torch.zeros(1, 1, odim, dtype=torch.float32, device=src_tokens.device)
+        ys = torch.zeros(1, 1, odim, dtype=torch.float32, device=dev)
         outs, probs, attns, idx = [], [], [], 0
         cache = None
         if kwargs.get("use_cache", False) in ("graph", "graph_body_eager"):
@@ -587,7 +596,7 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
             from ..incremental import synthesis_graph
             seed_t = RT._seed_t
             try:
-                sg = synthesis_graph(self, T_enc, max(maxlen, 1), src_tokens.device,
+                sg = synthesis_graph(self, T_enc, max(maxlen, 1), dev,
                                      capture=kwargs["use_cache"] == "graph")
                 before, stop_probs, attn = sg.synthesize(encoder_out, spkembs, threshold, minlen, maxlen)
                 return post.refine(before)[0], stop_probs, attn
@@ -792,6 +801,14 @@ def _check_sid_options(args):
         raise NotImplementedError("speaker identification with --use-codebook is not built")
     if not (getattr(args, "build_speech_encoder", False) and getattr(args, "build_text_decoder", False)):
         raise NotImplementedError("speaker identification needs --build-speech-encoder and --build-text-decoder")
+
+
+def _check_vc_options(args):
+    """The speech-enhancement variants of the s2s task (:917-918, 936-952) are not built: they fail at build time."""
+    if getattr(args, "se_predict", None) is not None:
+        raise NotImplementedError(f"--se-predict {args.se_predict} (speech enhancement) is not built")
+    if getattr(args, "se_decoder_input", "previous_target") != "previous_target":
+        raise NotImplementedError(f"--se-decoder-input {args.se_decoder_input} (speech enhancement) is not built")
 
 
 def make_args(arch="t5_transformer_base_asr", **overrides):

@@ -63,6 +63,12 @@ class Runtime:
         self._offset += 1
         return (self._offset | self.SEED_PTR_FLAG) if self._seed_t is not None else self._offset
 
+    def offset_block(self, base, i, width=64):
+        """LayerDrop stacks: the dropout draws of layer i start at offset base + i * width, whether or not earlier
+        layers ran. A captured update runs every layer and keeps or discards its output on the device, an eager one
+        skips the dropped layers; with fixed blocks the layers both run draw the same masks (a layer draws < width)."""
+        self._offset = base + i * width
+
     def manual_seed(self, seed):
         self._seed = int(seed)
         self._offset = 0

@@ -468,6 +468,12 @@ class B200Trainer:
             keep[i] = 1.0 if (np.random.random() > enc_p or i == unb) else 0.0
         for i in range(self._n_dec):
             keep[self._n_enc + i] = 1.0 if (dec_p <= 0 or torch.empty(1).uniform_().item() > dec_p) else 0.0
+        if self.device.type == "cuda":
+            # the copy runs when the stream reaches it, possibly after the NEXT update's draw: it reads a pinned block
+            # of its own, which the host allocator does not hand out again before the copy has completed
+            staged = torch.empty(keep.shape, dtype=keep.dtype, pin_memory=True)
+            staged.copy_(keep)
+            keep = staged
         self.layer_keep.copy_(keep, non_blocking=True)
         return True
 
@@ -477,7 +483,7 @@ class B200Trainer:
         here -- same stream, same order -- and hands them to forward() as explicit inputs."""
         prenet = getattr(self.model, "speech_encoder_prenet", None)
         ni = sample.get("net_input", {})
-        if (sample.get("task_name") not in ("s2t", "s2c") or prenet is None or not self.model.training or "mask_indices" in ni
+        if (sample.get("task_name") not in ("s2t", "s2c", "s2s") or prenet is None or not self.model.training or "mask_indices" in ni
                 or (prenet.mask_prob <= 0 and getattr(prenet, "mask_channel_prob", 0.0) <= 0)):
             return sample
         from .data import draw_hubert_masks
@@ -693,9 +699,13 @@ def pad_to_buckets(sample, buckets):
     out = dict(sample)
     ni = dict(sample["net_input"])
     task = sample.get("task_name", ni.get("task_name"))
-    if task == "t2s":
-        if "text" in buckets:
-            ni["src_tokens"] = pad_dim(ni["src_tokens"], 1, up(ni["src_tokens"].size(1), buckets["text"]), 1)
+    if task == "t2s" and "text" in buckets:
+        ni["src_tokens"] = pad_dim(ni["src_tokens"], 1, up(ni["src_tokens"].size(1), buckets["text"]), 1)
+    if task == "s2s" and "wave" in buckets:  # (data/speech_to_speech_dataset.py:169-228: waveform in, frames out)
+        n = up(ni["source"].size(1), buckets["wave"])
+        ni["source"] = pad_dim(ni["source"], 1, n, 0.0)
+        ni["padding_mask"] = pad_dim(ni["padding_mask"], 1, n, True)
+    if task in ("t2s", "s2s"):
         if "frames" in buckets:
             r = max(1, sample["dec_target"].size(1) // max(1, ni["prev_output_tokens"].size(1)))
             L = up(sample["dec_target"].size(1), buckets["frames"])
