@@ -172,6 +172,31 @@ typedef struct st5_attn_args {
 int st5_attn_fwd(const st5_attn_args* args, void* stream);
 int st5_attn_bwd(const st5_attn_args* args, void* stream);
 
+/* One-query-row attention of incremental decoding (forward only, fp32 math): the incremental path of
+ * multihead_attention.py:255-330 as the synthesis loop speecht5.py:1222-1245 runs it -- the decoder's self-attention
+ * over its key/value cache and its cross-attention over the encoder, one new row per (utterance b, head h).
+ *   q row of (b, h) at q[b * q_bs + h * 64 + c]; keys / values at k[b * k_bs + j * k_ld + h * 64 + c] (same for v);
+ *   out[b * o_bs + h * 64 + c] in `dtype` (ST5_F32 or ST5_BF16; q, k, v share it).
+ * key_pad [B][Tk] uint8 (or NULL): != 0 masks key j of utterance b; masked keys are never loaded. No relative positions,
+ * no causal mask, no dropout. probs (optional): the normalised fp32 probabilities, [B][H][Tk].
+ * Keys are reduced in fixed splits of 64 (split-KV over grid (splits, H, B), merged by a second launch when Tk > 64):
+ * a masked key adds an exact zero, so an utterance's result is bit-identical at any B and any key span Tk that holds
+ * its valid keys. ws: st5_attn_decode_ws_floats(B, H, Tk, probs != NULL) floats of scratch (none for Tk <= 64).
+ * K / V rows and strides must be 16-byte aligned. */
+typedef struct st5_attn_decode_args {
+  int32_t B, H, Tk, dtype;
+  const void* q; int64_t q_bs;
+  const void* k; int64_t k_ld, k_bs;
+  const void* v; int64_t v_ld, v_bs;
+  const uint8_t* key_pad;      /* [B][Tk] or NULL */
+  void* out; int64_t o_bs;
+  float* probs;                /* [B][H][Tk] or NULL */
+  float scale;
+  float* ws;
+} st5_attn_decode_args;
+int64_t st5_attn_decode_ws_floats(int32_t B, int32_t H, int32_t Tk, int32_t with_probs);
+int st5_attn_decode_fwd(const st5_attn_decode_args* args, void* stream);
+
 /* Fused wgmma attention forward (bf16, Tk <= 320): QK^T -> masks -> softmax -> dropout -> PV in ONE launch, no score
  * or probability round trip through HBM. Uses the q/k/v/out/probs/key_pad/scale/dropout fields of st5_attn_args exactly
  * like st5_attn_fwd; additionally writes lse[b][h][i] = log sum_j exp(scale*q_i.k_j) (may be NULL). probs (optional,

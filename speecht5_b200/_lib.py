@@ -47,6 +47,17 @@ class AttnArgs(C.Structure):
     ]
 
 
+class AttnDecodeArgs(C.Structure):
+    _fields_ = [
+        ("B", C.c_int32), ("H", C.c_int32), ("Tk", C.c_int32), ("dtype", C.c_int32),
+        ("q", C.c_void_p), ("q_bs", C.c_int64),
+        ("k", C.c_void_p), ("k_ld", C.c_int64), ("k_bs", C.c_int64),
+        ("v", C.c_void_p), ("v_ld", C.c_int64), ("v_bs", C.c_int64),
+        ("key_pad", C.c_void_p), ("out", C.c_void_p), ("o_bs", C.c_int64), ("probs", C.c_void_p),
+        ("scale", C.c_float), ("ws", C.c_void_p),
+    ]
+
+
 _vp, _i64, _i32, _f, _u64 = C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_uint64
 _PROTOS = {
     "st5_version": (C.c_int, []),
@@ -67,6 +78,8 @@ _PROTOS = {
     "st5_colsum": (C.c_int, [_vp, _i64, _vp, _i32, _i64, _i64, _i64, _i32, _vp]),
     "st5_attn_fwd": (C.c_int, [C.POINTER(AttnArgs), _vp]),
     "st5_attn_bwd": (C.c_int, [C.POINTER(AttnArgs), _vp]),
+    "st5_attn_decode_ws_floats": (C.c_int64, [_i32, _i32, _i32, _i32]),
+    "st5_attn_decode_fwd": (C.c_int, [C.POINTER(AttnDecodeArgs), _vp]),
     "st5_attn_fused_fwd": (C.c_int, [C.POINTER(AttnArgs), _vp, _vp, _vp, _vp, _vp]),
     "st5_attn_flash_fwd": (C.c_int, [C.POINTER(AttnArgs), _vp, _vp, _vp, _vp, _vp]),
     "st5_attn_fused_bwd": (C.c_int, [C.POINTER(AttnArgs), _vp, _vp, _vp, _vp, _vp, _i32, _vp]),

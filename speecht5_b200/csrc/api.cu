@@ -130,6 +130,12 @@ int st5_attn_fwd(const st5_attn_args* a, void* stream) {
 int st5_attn_bwd(const st5_attn_args* a, void* stream) {
   return set_error(attn_bwd_launch(*a, (cudaStream_t)stream), "st5_attn_bwd");
 }
+int64_t st5_attn_decode_ws_floats(int32_t B, int32_t H, int32_t Tk, int32_t with_probs) {
+  return attn_decode_ws_floats(B, H, Tk, with_probs);
+}
+int st5_attn_decode_fwd(const st5_attn_decode_args* a, void* stream) {
+  return set_error(attn_decode_launch(*a, (cudaStream_t)stream), "st5_attn_decode_fwd");
+}
 
 int st5_bn_fwd(const void* x, int64_t x_ld, const float* gamma, const float* beta, float* running_mean,
                float* running_var, float* save_mean, float* save_rstd, void* y, int64_t y_ld, void* y_pre, int dtype,

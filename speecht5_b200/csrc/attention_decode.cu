@@ -1,0 +1,203 @@
+// One-query-row attention for incremental decoding: the decoder's self-attention over its key/value cache and its
+// cross-attention over the encoder, one new row per (utterance, head) and step.
+//
+// Reference: the incremental path of speecht5/models/modules/multihead_attention.py:255-330 (saved prev_key /
+// prev_value, one query row) inside the synthesis loop of speecht5/models/speecht5.py:1222-1245.
+//
+// Split-KV: the keys of an utterance are cut into fixed splits of DCH keys. Each CTA of grid (splits, H, B) reduces one
+// split to (max, sum of exponentials, 64-wide unnormalised accumulator); a combine kernel merges the splits in index
+// order. Key j always lands in split j / DCH at the same lane position, and a masked key adds an exact zero (a split
+// whose keys are all masked merges with weight zero), so an utterance's result depends only on its own valid keys: not
+// on B and not on the buffer's key span (the bucket of a captured graph).
+#include "kernels.cuh"
+
+namespace st5 {
+
+constexpr int DT = 128;   // threads per CTA
+constexpr int DH = 64;    // head dim
+constexpr int DCH = 64;   // keys per split
+constexpr int DPART = DH + 2;  // partial record: max, sum, accumulator[64]
+
+__device__ __forceinline__ float* decode_probs(const st5_attn_decode_args& a, int b, int h) {
+  return a.probs != nullptr ? a.probs + ((int64_t)b * a.H + h) * a.Tk : nullptr;
+}
+
+template <typename T> struct Vec16;
+template <> struct Vec16<float> {
+  static constexpr int N = 4;
+  static __device__ __forceinline__ void load(const float* p, float* o) {
+    const float4 v = *reinterpret_cast<const float4*>(p);
+    o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
+  }
+};
+template <> struct Vec16<__nv_bfloat16> {
+  static constexpr int N = 8;
+  static __device__ __forceinline__ void load(const __nv_bfloat16* p, float* o) {
+    const uint4 v = *reinterpret_cast<const uint4*>(p);
+    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v);
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const float2 f = __bfloat1622float2(h[t]);
+      o[2 * t] = f.x; o[2 * t + 1] = f.y;
+    }
+  }
+};
+
+__device__ __forceinline__ float cta_reduce(float v, float* red, bool is_max) {
+  v = is_max ? warp_max(v) : warp_sum(v);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float r = red[0];
+#pragma unroll
+  for (int w = 1; w < DT / 32; ++w) r = is_max ? fmaxf(r, red[w]) : r + red[w];
+  return r;
+}
+
+// direct != 0: the buffer holds at most DCH keys, so there is one split and this CTA writes the final output (and
+// probabilities) itself -- bit-identical to what the combine kernel makes of a single split.
+template <typename T>
+__global__ void __launch_bounds__(DT) attn_decode_split(const st5_attn_decode_args a, int n_splits, int direct) {
+  constexpr int VE = Vec16<T>::N;   // elements per 16-byte load
+  constexpr int LPK = DH / VE;      // lanes per key row
+  constexpr int KPI = DT / LPK;     // keys per CTA iteration
+  __shared__ float q[DH];
+  __shared__ float sc[DCH];
+  __shared__ float red[DT / 32];
+  __shared__ float part[DT / 32][DH];
+  const int s = blockIdx.x, h = blockIdx.y, b = blockIdx.z, tid = threadIdx.x;
+  const int j0 = s * DCH;
+  const int j1 = min(j0 + DCH, a.Tk);
+  if (tid < DH) q[tid] = ldf((const T*)a.q + (int64_t)b * a.q_bs + h * DH + tid);
+  __syncthreads();
+  const int lane = tid & 31, sub = lane % LPK, slot = tid / LPK;
+  float qr[VE];
+#pragma unroll
+  for (int e = 0; e < VE; ++e) qr[e] = q[sub * VE + e];
+  const uint8_t* kp = a.key_pad != nullptr ? a.key_pad + (int64_t)b * a.Tk : nullptr;
+  const T* kb = (const T*)a.k + (int64_t)b * a.k_bs + h * DH + sub * VE;
+#pragma unroll
+  for (int it = 0; it < DCH / KPI; ++it) {
+    const int j = j0 + it * KPI + slot;
+    const bool valid = j < j1 && (kp == nullptr || kp[j] == 0);
+    float d = 0.f;
+    if (valid) {
+      float kr[VE];
+      Vec16<T>::load(kb + (int64_t)j * a.k_ld, kr);
+#pragma unroll
+      for (int e = 0; e < VE; ++e) d += qr[e] * kr[e];
+    }
+#pragma unroll
+    for (int o = LPK / 2; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+    if (sub == 0) sc[j - j0] = valid ? d * a.scale : -INFINITY;
+  }
+  __syncthreads();
+  const float sraw = tid < DCH ? sc[tid] : -INFINITY;
+  const float m = cta_reduce(sraw, red, true);
+  const float ex = sraw == -INFINITY ? 0.f : expf(sraw - m);  // (a split with every key masked: m = -inf, all zero)
+  const float l = cta_reduce(ex, red, false);
+  if (tid < DCH) sc[tid] = ex;
+  const int64_t bh = (int64_t)b * a.H + h;
+  if (!direct && a.probs != nullptr && tid < DCH && j0 + tid < a.Tk) a.ws[(int64_t)n_splits * DPART * a.B * a.H + bh * a.Tk + j0 + tid] = sraw;
+  __syncthreads();
+  // out_c = sum_j e_j v_jc: lane `sub` owns channels sub*VE .. +VE, slots stride over the split's keys
+  const T* vb = (const T*)a.v + (int64_t)b * a.v_bs + h * DH + sub * VE;
+  float acc[VE];
+#pragma unroll
+  for (int e = 0; e < VE; ++e) acc[e] = 0.f;
+#pragma unroll
+  for (int it = 0; it < DCH / KPI; ++it) {
+    const int jj = it * KPI + slot;
+    const float p = sc[jj];
+    if (j0 + jj < j1 && p != 0.f) {
+      float vr[VE];
+      Vec16<T>::load(vb + (int64_t)(j0 + jj) * a.v_ld, vr);
+#pragma unroll
+      for (int e = 0; e < VE; ++e) acc[e] += p * vr[e];
+    }
+  }
+#pragma unroll
+  for (int e = 0; e < VE; ++e) {
+#pragma unroll
+    for (int o = LPK; o < 32; o <<= 1) acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], o);
+  }
+  if (lane < LPK) {
+#pragma unroll
+    for (int e = 0; e < VE; ++e) part[tid >> 5][sub * VE + e] = acc[e];
+  }
+  __syncthreads();
+  if (tid < DH) {
+    float r = part[0][tid];
+#pragma unroll
+    for (int w = 1; w < DT / 32; ++w) r += part[w][tid];
+    if (direct) {
+      stf((T*)a.out + (int64_t)b * a.o_bs + h * DH + tid, r * (1.f / l));
+    } else {
+      float* pr = a.ws + (bh * n_splits + s) * DPART;
+      pr[2 + tid] = r;
+      if (tid == 0) { pr[0] = m; pr[1] = l; }
+    }
+  }
+  if (direct) {
+    float* pr = decode_probs(a, b, h);
+    if (pr != nullptr) {
+      const float inv = 1.f / l;
+      for (int j = tid; j < a.Tk; j += DT) pr[j] = sc[j] * inv;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(DT) attn_decode_combine(const st5_attn_decode_args a, int n_splits, int dtype) {
+  const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  const int ns = n_splits;
+  const int64_t bh = (int64_t)b * a.H + h;
+  const float* pr = a.ws + bh * n_splits * DPART;
+  float M = -INFINITY;
+  for (int s = 0; s < ns; ++s) M = fmaxf(M, pr[s * DPART]);
+  float L = 0.f;
+  for (int s = 0; s < ns; ++s) {
+    const float ms = pr[s * DPART];
+    L += ms == -INFINITY ? 0.f : pr[s * DPART + 1] * expf(ms - M);
+  }
+  const float inv = 1.f / L;
+  if (tid < DH) {
+    float r = 0.f;
+    for (int s = 0; s < ns; ++s) {
+      const float ms = pr[s * DPART];
+      r += pr[s * DPART + 2 + tid] * (ms == -INFINITY ? 0.f : expf(ms - M));
+    }
+    r *= inv;
+    if (dtype == ST5_F32) stf((float*)a.out + (int64_t)b * a.o_bs + h * DH + tid, r);
+    else stf((__nv_bfloat16*)a.out + (int64_t)b * a.o_bs + h * DH + tid, r);
+  }
+  float* po = decode_probs(a, b, h);
+  if (po != nullptr) {
+    const float* sr = a.ws + (int64_t)n_splits * DPART * a.B * a.H + bh * a.Tk;
+    for (int j = tid; j < a.Tk; j += DT) po[j] = sr[j] == -INFINITY ? 0.f : expf(sr[j] - M) * inv;
+  }
+}
+
+int64_t attn_decode_ws_floats(int B, int H, int Tk, int with_probs) {
+  if (Tk <= DCH) return 0;
+  const int64_t ns = (Tk + DCH - 1) / DCH;
+  return (int64_t)B * H * (ns * DPART + (with_probs ? Tk : 0));
+}
+
+int attn_decode_launch(const st5_attn_decode_args& a, cudaStream_t st) {
+  if (a.B <= 0 || a.H <= 0 || a.Tk <= 0) return -2;
+  const int esz = a.dtype == ST5_F32 ? 4 : 2;
+  if (((a.k_ld * esz) & 15) || ((a.v_ld * esz) & 15) || ((a.k_bs * esz) & 15) || ((a.v_bs * esz) & 15)) return -6;
+  if ((reinterpret_cast<uintptr_t>(a.k) & 15) || (reinterpret_cast<uintptr_t>(a.v) & 15)) return -6;
+  const int ns = (a.Tk + DCH - 1) / DCH;
+  const int direct = ns == 1;
+  if (!direct && a.ws == nullptr) return -5;
+  const dim3 grid(ns, a.H, a.B);
+  if (a.dtype == ST5_F32) attn_decode_split<float><<<grid, DT, 0, st>>>(a, ns, direct);
+  else attn_decode_split<__nv_bfloat16><<<grid, DT, 0, st>>>(a, ns, direct);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess || direct) return (int)e;
+  attn_decode_combine<<<dim3(a.H, a.B), DT, 0, st>>>(a, ns, a.dtype);
+  return (int)cudaGetLastError();
+}
+
+}  // namespace st5

@@ -145,6 +145,8 @@ int colsum_launch(const void* x, int64_t ld, float* out, int dtype, int64_t rows
                   int accumulate, cudaStream_t s);
 int attn_fwd_launch(const st5_attn_args& a, cudaStream_t s);
 int attn_bwd_launch(const st5_attn_args& a, cudaStream_t s);
+int64_t attn_decode_ws_floats(int B, int H, int Tk, int with_probs);
+int attn_decode_launch(const st5_attn_decode_args& a, cudaStream_t s);
 int bn_fwd_launch(const void* x, int64_t x_ld, const float* gamma, const float* beta, float* running_mean,
                   float* running_var, float* save_mean, float* save_rstd, void* y, int64_t y_ld, void* y_pre, int dtype,
                   int64_t rows, int64_t C, int training, float momentum, float eps, int act, float drop_p,

@@ -8,7 +8,8 @@ device (tests/test_frontend_gpu.py); nothing on the training path imports this m
 Per utterance batch the cross-attention keys / values of every decoder layer are projected ONCE; every step projects
 q | k | v of the single new row, appends k | v to the layer's [B, T_max, 2C] cache and attends over the cache with a
 one-row query -- O(L) work per step instead of the O(L^2) prefix recomputation. All contractions run on the existing
-GEMM, the one-row attention on the exact row kernels (st5_attn_fwd), which take strided key / value views."""
+GEMM, the one-row attention on the split-KV decode kernel (st5_attn_decode_fwd), which takes strided key / value
+views."""
 import torch
 
 from . import ops
@@ -20,13 +21,13 @@ def _act_dtype(x):
 
 
 def _attend(*a, **kw):
-    """One-row queries: the row kernels (the fused wgmma path works on 64-query tiles)."""
-    prev = RT.attn_tensor_core
-    RT.attn_tensor_core = False
+    """One-row queries: the split-KV decode kernel (st5_attn_decode_fwd; the fused wgmma path works on 64-query tiles)."""
+    prev = RT.attn_decode_rows
+    RT.attn_decode_rows = True
     try:
         return ops.attention(*a, **kw)
     finally:
-        RT.attn_tensor_core = prev
+        RT.attn_decode_rows = prev
 
 
 class DecoderCache:
@@ -118,45 +119,53 @@ class _StaticCache:
 
 
 class SynthesisGraph:
-    """Greedy speech synthesis (models/speecht5.py:1188-1249) with every decoder step = ONE CUDA-graph replay: prenet on
-    the newest frame (always-on dropout drawn from the device-resident seed, advanced inside the graph), positional row
-    gathered by the device step counter, the key/value-cached decoder, feat_out | prob_out, and the step's outputs
-    written into preallocated result buffers at the step index.
+    """Greedy speech synthesis (models/speecht5.py:1188-1249) of B utterances at once, with every decoder step = ONE
+    CUDA-graph replay: prenet on each utterance's newest frame (always-on dropout drawn from the device-resident seed,
+    advanced inside the graph), positional row gathered by the device step counter, the key/value-cached decoder,
+    feat_out | prob_out, each utterance's stopping rule, and the step's outputs written into preallocated result buffers
+    at the step index. B = 1 is generate_speech(use_cache="graph"); generate_speech_batch uses any B.
 
     The object is utterance-independent and is kept on the model (`synthesis_graph`): every buffer a graph reads has a
-    fixed size -- the cross-attention keys / values of an utterance are copied into [1, S_bucket, 2C] buffers with the
-    tail masked, the frame budget is a bucket too -- so the graphs captured for one utterance serve every later one of
-    the same buckets (serving: no capture on the request path after the first). Self-attention spans are bucketed (128,
-    256, ...): one graph per span, so a step attends over at most 2x the keys it needs. The host replays `chunk` steps,
-    then reads their stop flags in one copy (the reference's `int(sum(probs[-1] >= threshold)) > 0`, :1235); steps
-    replayed past the stopping one are discarded."""
+    fixed size -- the cross-attention keys / values of utterance b are copied into row b of [B, S_bucket, 2C] buffers
+    with the tail masked, the frame budget is a bucket too -- so the graphs captured for one batch serve every later one
+    of the same buckets (serving: no capture on the request path after the first). Self-attention spans are bucketed
+    (128, 256, ...): one graph per span, so a step attends over at most 2x the keys it needs. Every row keeps the
+    reference's stopping rule (:1235-1245) with its own minlen / maxlen; the done flags and lengths are device tensors
+    written inside the graph. The host replays `chunk` steps, then reads their "all done" flags in one copy; rows that
+    finished earlier keep running and what they compute past their length is discarded."""
 
     CHUNK = 8
 
-    def __init__(self, model, S_bucket, maxlen_bucket, device, capture=True):
+    def __init__(self, model, S_bucket, maxlen_bucket, device, capture=True, B=1, attention=True):
         self.m = model
         self.capture = capture  # False: the same step body runs eagerly (CPU checks of the device-counter form)
         dec, post = model.decoder, model.speech_decoder_postnet
         dev = torch.device(device)
         self.dev, self.r, self.odim = dev, model.reduction_factor, post.odim
-        self.S, self.maxlen = int(S_bucket), int(maxlen_bucket)
+        self.B, self.S, self.maxlen = int(B), int(S_bucket), int(maxlen_bucket)
+        B = self.B
         rows = self.maxlen + self.CHUNK
         L, H = len(dec.layers), dec.layers[0].encoder_attn.num_heads
         C = dec.layers[0].self_attn.embed_dim
-        self.cache = _StaticCache([torch.zeros((1, self.S, 2 * C), dtype=RT.dtype, device=dev) for _ in dec.layers],
-                                  [torch.zeros((1, rows, 2 * C), dtype=RT.dtype, device=dev) for _ in dec.layers],
-                                  torch.zeros((1, self.S), dtype=torch.uint8, device=dev), rows)
+        self.cache = _StaticCache([torch.zeros((B, self.S, 2 * C), dtype=RT.dtype, device=dev) for _ in dec.layers],
+                                  [torch.zeros((B, rows, 2 * C), dtype=RT.dtype, device=dev) for _ in dec.layers],
+                                  torch.zeros((B, self.S), dtype=torch.uint8, device=dev), rows)
         self.t = torch.zeros(1, dtype=torch.int64, device=dev)
-        self.ys_last = torch.zeros(1, 1, self.odim, dtype=torch.float32, device=dev)
-        self.outs = torch.zeros(rows, self.r, self.odim, dtype=torch.float32, device=dev)
-        self.probs = torch.zeros(rows, self.r, dtype=torch.float32, device=dev)
-        self.attn = torch.zeros(rows, L, H, self.S, dtype=torch.float32, device=dev)
-        self.stop = torch.zeros(rows, dtype=torch.int32, device=dev)
+        self.ys_last = torch.zeros(B, 1, self.odim, dtype=torch.float32, device=dev)
+        self.outs = torch.zeros(rows, B, self.r, self.odim, dtype=torch.float32, device=dev)
+        self.probs = torch.zeros(rows, B, self.r, dtype=torch.float32, device=dev)
+        # the cross-attention record is opt-in: [rows, B, layers, H, S] fp32 is 3.6 GiB per 30 s utterance
+        self.attn = torch.zeros(rows, B, L, H, self.S, dtype=torch.float32, device=dev) if attention else None
+        self.stop = torch.zeros(rows, dtype=torch.int32, device=dev)  # every row done after step t
+        self.done = torch.zeros(B, dtype=torch.bool, device=dev)
+        self.lengths = torch.zeros(B, dtype=torch.int64, device=dev)
+        self.minlen = torch.zeros(B, dtype=torch.int64, device=dev)
+        self.maxlen_b = torch.zeros(B, dtype=torch.int64, device=dev)
         self.threshold = torch.full((1,), 0.5, dtype=torch.float32, device=dev)
         self.pos = torch.arange(rows, device=dev)
         pre = model.speech_decoder_prenet
         self.pe = pre.decoder_prenet[1].table(rows, dev)
-        self.spk_bias = torch.zeros((1, pre.embed_dim), dtype=torch.float32, device=dev)
+        self.spk_bias = torch.zeros((B, pre.embed_dim), dtype=torch.float32, device=dev)
         self.with_spk = False
         self.graphs = {}
         self.stream = torch.cuda.Stream(device=dev) if capture else None
@@ -166,21 +175,26 @@ class SynthesisGraph:
         self.seed_t = torch.zeros(1, dtype=torch.int64, device=dev)
 
     @torch.no_grad()
-    def begin(self, encoder_out, spkembs, threshold):
-        """Load one utterance: project its cross-attention keys / values into the static buffers, reset the counters."""
-        enc = encoder_out.get("_encoder_out_btc")
-        if enc is None:
-            enc = encoder_out["encoder_out"][0].transpose(0, 1).contiguous()
-        enc = _act_dtype(enc)
-        S = enc.shape[1]
-        assert enc.shape[0] == 1 and S <= self.S and RT.dtype == self.dtype
-        pm = encoder_out["encoder_padding_mask"]
+    def begin(self, encoder_outs, spkembs, threshold, minlens, maxlens):
+        """Load B utterances (one encoder output each, batch 1): project their cross-attention keys / values into rows
+        of the static buffers, set their length limits, reset the counters. Returns their encoder lengths."""
+        assert len(encoder_outs) == self.B and RT.dtype == self.dtype
         self.cache.enc_pad.fill_(1)
-        self.cache.enc_pad[:, :S] = pm[0].to(torch.uint8) if len(pm) > 0 and pm[0] is not None else 0
-        for li, layer in enumerate(self.m.decoder.layers):
-            ca = layer.encoder_attn
-            self.cache.cross[li][:, :S] = ops.linear(enc, (ca.k_proj.weight, ca.v_proj.weight),
-                                                     (ca.k_proj.bias, ca.v_proj.bias))
+        lens = []
+        for b, encoder_out in enumerate(encoder_outs):
+            enc = encoder_out.get("_encoder_out_btc")
+            if enc is None:
+                enc = encoder_out["encoder_out"][0].transpose(0, 1).contiguous()
+            enc = _act_dtype(enc)
+            S = enc.shape[1]
+            assert enc.shape[0] == 1 and S <= self.S
+            pm = encoder_out["encoder_padding_mask"]
+            self.cache.enc_pad[b, :S] = pm[0][0].to(torch.uint8) if len(pm) > 0 and pm[0] is not None else 0
+            for li, layer in enumerate(self.m.decoder.layers):
+                ca = layer.encoder_attn
+                self.cache.cross[li][b:b + 1, :S] = ops.linear(enc, (ca.k_proj.weight, ca.v_proj.weight),
+                                                               (ca.k_proj.bias, ca.v_proj.bias))
+            lens.append(S)
         pre = self.m.speech_decoder_prenet
         with_spk = spkembs is not None
         if self.graphs and with_spk != self.with_spk:
@@ -191,13 +205,17 @@ class SynthesisGraph:
             spk = torch.nn.functional.normalize(spkembs.float()).to(RT.dtype)
             self.spk_bias.copy_(ops.linear(spk, W[:, d:], (), out_dtype=torch.float32, key=("spk_w", id(W)), need_dx=False))
         self.threshold.fill_(float(threshold))
+        self.minlen.copy_(torch.tensor(minlens, dtype=torch.int64))
+        self.maxlen_b.copy_(torch.tensor(maxlens, dtype=torch.int64))
+        self.done.zero_()
+        self.lengths.zero_()
         self.t.zero_()
         self.ys_last.zero_()
         if self.capture:
-            self.seed_t.fill_(RT._seed + (RT._draws << 20))  # a fresh stream of prenet masks per utterance
+            self.seed_t.fill_(RT._seed + (RT._draws << 20))  # a fresh stream of prenet masks per batch
             RT._draws += 1
             RT._seed_t = self.seed_t
-        return S
+        return lens
 
     def _body(self, span):
         m, pre, post = self.m, self.m.speech_decoder_prenet, self.m.speech_decoder_postnet
@@ -210,16 +228,25 @@ class SynthesisGraph:
         if self.with_spk:
             W, b, d = pre.spkembs_layer[0].weight, pre.spkembs_layer[0].bias, pre.embed_dim
             x = ops.linear(x, W[:, :d], b, act="relu", bias2=self.spk_bias, bias2_rows=1, key=("spk_h", id(W)))
-        self_pad = (self.pos[:span] > self.t).to(torch.uint8)[None].contiguous()
-        z, layer_attn = decoder_step(m.decoder, x, self.cache, need_head_weights=True, t_dev=self.t, span=span,
+        self_pad = (self.pos[:span] > self.t).to(torch.uint8)[None].expand(self.B, span).contiguous()
+        want = self.attn is not None
+        z, layer_attn = decoder_step(m.decoder, x, self.cache, need_head_weights=want, t_dev=self.t, span=span,
                                      self_pad=self_pad)
-        before, logits = post.project(z.contiguous())  # [1, r, odim], [1, r]
+        before, logits = post.project(z.contiguous())  # [B, r, odim], [B, r]
         p = torch.sigmoid(logits)
-        self.outs.index_copy_(0, self.t, before)
-        self.probs.index_copy_(0, self.t, p)
-        self.attn.index_copy_(0, self.t, torch.stack([a[0, :, 0, :] for a in layer_attn], 0)[None])
+        self.outs.index_copy_(0, self.t, before[None])
+        self.probs.index_copy_(0, self.t, p[None])
+        if want:
+            self.attn.index_copy_(0, self.t, torch.stack([a[:, :, 0, :] for a in layer_attn], 1)[None])
         self.ys_last.copy_(before[:, -1:, :])
-        self.stop.index_copy_(0, self.t, (p >= self.threshold).any().to(torch.int32).reshape(1))
+        # (:1235-1245) per row: stop once a probability of the group reaches the threshold or idx >= maxlen, but not
+        # before idx >= minlen; idx = t + 1 is the reference's counter after this step
+        i = self.t + 1
+        fin = ((p >= self.threshold).any(-1) | (i >= self.maxlen_b)) & (i >= self.minlen)
+        newly = fin & ~self.done
+        self.lengths.copy_(torch.where(newly, i.expand(self.B), self.lengths))
+        self.done |= newly
+        self.stop.index_copy_(0, self.t, self.done.all().to(torch.int32).reshape(1))
         self.t += 1
         RT.advance_seed()
 
@@ -231,11 +258,13 @@ class SynthesisGraph:
 
     def _snapshot(self):
         """State the step body overwrites that a replay of the same step does not rewrite first (capture warm-up)."""
-        keep = self.ys_last.clone()
+        keep, done, lengths = self.ys_last.clone(), self.done.clone(), self.lengths.clone()
 
         def undo():
             self.seed_t -= 1  # (the pass drew from the seed the replay of this step must see)
             self.ys_last.copy_(keep)
+            self.done.copy_(done)
+            self.lengths.copy_(lengths)
         return undo
 
     @torch.no_grad()
@@ -266,44 +295,44 @@ class SynthesisGraph:
         return self.stop[t0:t0 + n].tolist()
 
     @torch.no_grad()
-    def synthesize(self, encoder_out, spkembs, threshold, minlen, maxlen):
-        """The reference's loop (:1222-1249): returns (before frames [1, L, odim], stop probabilities [L], attention
-        [layers, H, L/r, S])."""
-        assert maxlen <= self.maxlen
-        minlen = min(minlen, max(maxlen, 1))  # (the reference's loop has no exit past maxlen frames otherwise)
-        S = self.begin(encoder_out, spkembs, threshold)
+    def synthesize(self, encoder_outs, spkembs, threshold, minlens, maxlens):
+        """The reference's loop (:1222-1249) for every row: returns one (before frames [1, L_b, odim], stop
+        probabilities [L_b], attention [layers, H, L_b/r, S_b] or None) per utterance."""
+        assert max(maxlens) <= self.maxlen
+        # (the reference's loop has no exit past maxlen frames otherwise)
+        minlens = [min(mn, max(mx, 1)) for mn, mx in zip(minlens, maxlens)]
+        S = self.begin(encoder_outs, spkembs, threshold, minlens, maxlens)
+        last = max(max(mx, 1) for mx in maxlens)  # every row is done after this many steps
         idx = 0
         while True:
-            n = max(1, min(self.CHUNK, max(maxlen, 1) - idx))
+            n = max(1, min(self.CHUNK, last - idx))
             flags = self.run(idx, n)
-            done = None
-            for k, f in enumerate(flags):
-                i = idx + k + 1  # the reference's idx after this step
-                if (f or i >= maxlen) and i >= minlen:
-                    done = i
-                    break
-            if done is not None:
-                idx = done
-                break
             idx += n
-        return (self.outs[:idx].reshape(1, idx * self.r, self.odim).clone(), self.probs[:idx].reshape(-1).clone(),
-                self.attn[:idx, :, :, :S].permute(1, 2, 0, 3).contiguous())
+            if any(flags):
+                break
+        res = []
+        for b, L in enumerate(self.lengths.tolist()):
+            attn = self.attn[:L, b, :, :, :S[b]].permute(1, 2, 0, 3).contiguous() if self.attn is not None else None
+            res.append((self.outs[:L, b].reshape(1, L * self.r, self.odim).clone(), self.probs[:L, b].reshape(-1).clone(),
+                        attn))
+        return res
 
 
-def synthesis_graph(model, S, maxlen, device, capture=True):
-    """The model's SynthesisGraph for text length S and a frame budget of maxlen decoder steps (buckets: S to multiples of
-    64, maxlen to powers of two >= 256); rebuilt when the numeric mode or the weights' owner changed."""
+def synthesis_graph(model, S, maxlen, device, capture=True, B=1, attention=True):
+    """The model's SynthesisGraph for B utterances, encoder length S and a frame budget of maxlen decoder steps
+    (buckets: S to multiples of 64, maxlen to powers of two >= 256); rebuilt when the numeric mode or the weights'
+    owner changed."""
     S_b = max(64, (S + 63) // 64 * 64)
     M_b = 256
     while M_b < maxlen:
         M_b *= 2
     store = model.__dict__.setdefault("_synthesis_graphs", {})
-    key = (S_b, M_b, RT.dtype, str(device), bool(capture), RT.param_epoch)
+    key = (B, bool(attention), S_b, M_b, RT.dtype, str(device), bool(capture), RT.param_epoch)
     sg = store.get(key)
     if sg is None:
-        for k in [k for k in store if k[:5] == key[:5]]:  # same buckets, stale weights
+        for k in [k for k in store if k[:7] == key[:7]]:  # same buckets, stale weights
             del store[k]
-        sg = store[key] = SynthesisGraph(model, S_b, M_b, device, capture=capture)
+        sg = store[key] = SynthesisGraph(model, S_b, M_b, device, capture=capture, B=B, attention=attention)
     return sg
 
 

@@ -195,6 +195,28 @@ def attn_fwd(a):
     _count(1)
 
 
+def attn_decode_fwd(q, k, v, out, *, H, scale, key_pad=None, probs=None):
+    """st5_attn_decode_fwd (include/speecht5_b200.h): one query row per (utterance, head). q [B, 1, H*64] and
+    k / v [B, Tk, H*64] are strided views (e.g. column blocks of a fused projection buffer), out [B, 1, H*64];
+    probs (optional) a contiguous fp32 [B, H, 1, Tk] tensor that receives the probabilities."""
+    _require_cuda(q, k, v, out, key_pad, probs)
+    assert q.dtype == k.dtype == v.dtype == out.dtype and k.stride(2) == 1 and v.stride(2) == 1
+    B, Tk = k.shape[0], k.shape[1]
+    assert probs is None or (probs.dtype == torch.float32 and probs.is_contiguous() and probs.numel() == B * H * Tk)
+    lib = _lib.load()
+    nws = lib.st5_attn_decode_ws_floats(B, H, Tk, int(probs is not None))
+    ws = torch.empty(nws, dtype=torch.float32, device=out.device) if nws > 0 else None
+    a = _lib.AttnDecodeArgs()
+    a.B, a.H, a.Tk, a.dtype = B, H, Tk, dtype_id(out)
+    a.q, a.q_bs = q.data_ptr(), q.stride(0)
+    a.k, a.k_ld, a.k_bs = k.data_ptr(), k.stride(1), k.stride(0)
+    a.v, a.v_ld, a.v_bs = v.data_ptr(), v.stride(1), v.stride(0)
+    a.key_pad, a.out, a.o_bs, a.probs = _ptr(key_pad), out.data_ptr(), out.stride(0), _ptr(probs)
+    a.scale, a.ws = scale, _ptr(ws)
+    _lib.check(lib.st5_attn_decode_fwd(C.byref(a), _stream()), "st5_attn_decode_fwd")
+    _count(1 if nws == 0 else 2)
+
+
 def attn_bwd(a):
     lib = _lib.load()
     _lib.check(lib.st5_attn_bwd(C.byref(a), _stream()), "st5_attn_bwd")

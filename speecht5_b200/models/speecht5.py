@@ -598,7 +598,7 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
             try:
                 sg = synthesis_graph(self, T_enc, max(maxlen, 1), dev,
                                      capture=kwargs["use_cache"] == "graph")
-                before, stop_probs, attn = sg.synthesize(encoder_out, spkembs, threshold, minlen, maxlen)
+                before, stop_probs, attn = sg.synthesize([encoder_out], spkembs, threshold, [minlen], [maxlen])[0]
                 return post.refine(before)[0], stop_probs, attn
             finally:
                 RT._seed_t = seed_t
@@ -624,6 +624,55 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
                     continue
                 mel = post.refine(torch.cat(outs, dim=0).unsqueeze(0))[0]
                 return mel, torch.cat(probs, dim=0), torch.cat(attns, dim=2)
+
+    @torch.no_grad()
+    def generate_speech_batch(self, src_tokens=None, src_lengths=None, source=None, padding_mask=None, spkembs=None,
+                              attention=False, **kwargs):
+        """generate_speech for a batch: each utterance gets exactly what generate_speech(use_cache="graph") gives it
+        alone (same knobs, defaults and `threshold` quirk; maxlen / minlen from the utterance's own encoder length),
+        with ONE decoder step of all utterances per CUDA-graph replay (incremental.SynthesisGraph).
+
+        Text input: src_tokens [B, T] padded, src_lengths [B] (None: no padding). Speech input: source [B, N] padded,
+        padding_mask [B, N] (True = padding; None: no padding). spkembs [B, spk_dim] or None. The encoders and the
+        post-net refinement run per utterance on its unpadded input: the speech front end's first GroupNorm normalises
+        over all time steps and the post-net's k5 convolutions read neighbouring frames, so padding would change both.
+        Returns a list of (mel [L_b, odim], stop probabilities [L_b * r], cross-attention [layers, H, L_b / r, T_b] when
+        attention=True else None). use_cache: "graph" (default) or "graph_body_eager" (the same step body, eagerly)."""
+        assert (source is None) != (src_tokens is None)
+        if spkembs is not None and getattr(self.args, "spk_embed_integration_type", "pre") != "pre":
+            raise NotImplementedError("spk_embed_integration_type != 'pre'")
+        mode = kwargs.get("use_cache", "graph")
+        if mode not in ("graph", "graph_body_eager"):
+            raise ValueError(f"generate_speech_batch decodes through the captured step only (use_cache={mode!r})")
+        threshold = kwargs.get("threshold", 0.5)
+        minlenratio = kwargs.get("threshold", 0.0)
+        maxlenratio = kwargs.get("threshold", 20.0 if source is None else 10.0)
+        x = src_tokens if source is None else source
+        B, dev = x.size(0), x.device
+        encs, minlens, maxlens = [], [], []
+        for b in range(B):
+            if source is None:
+                n = int(src_lengths[b]) if src_lengths is not None else src_tokens.size(1)
+                enc = self.forward_text_encoder(src_tokens[b:b + 1, :n])
+            else:
+                n = int((~padding_mask[b]).sum()) if padding_mask is not None else source.size(1)
+                enc = self.forward_encoder(source[b:b + 1, :n],
+                                           padding_mask=padding_mask[b:b + 1, :n] if padding_mask is not None else None)
+            T_enc = enc["encoder_out"][0].size(0)
+            encs.append(enc)
+            maxlens.append(int(T_enc * maxlenratio / self.reduction_factor))
+            minlens.append(int(T_enc * minlenratio / self.reduction_factor))
+        from ..incremental import synthesis_graph
+        S = max(e["encoder_out"][0].size(0) for e in encs)
+        seed_t = RT._seed_t
+        try:
+            sg = synthesis_graph(self, S, max(max(m, 1) for m in maxlens), dev, capture=mode == "graph", B=B,
+                                 attention=attention)
+            res = sg.synthesize(encs, spkembs, threshold, minlens, maxlens)
+        finally:
+            RT._seed_t = seed_t
+        post = self.speech_decoder_postnet
+        return [(post.refine(before)[0], probs, attn) for before, probs, attn in res]
 
 
 # ---------------------------------------------------------------------------------------------- architectures

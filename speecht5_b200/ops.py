@@ -33,6 +33,8 @@ class Runtime:
         self.attn_tensor_core = True  # bf16 mode: contractions of attention on the wgmma GEMM (else row kernels)
         self.attn_fused = True        # bf16 mode, Tk <= 320: single-launch fused forward (attention_flash.cu)
         self.attn_fused_bwd = True    # ... and the flash-style fused backward (attention_fused_bwd.cu)
+        # set by incremental._attend: one-row, no-grad queries go to the split-KV decode kernel (attention_decode.cu)
+        self.attn_decode_rows = False
         self.fold_residual_grad = os.environ.get("ST5_FOLD_RESGRAD", "1") != "0"  # see LinearFn.forward (passthrough)
         self.probs_grad_heads = 0     # > 0: gradients on returned probabilities exist for the first n heads only
         self.probs_read_heads = 0     # > 0: nobody READS returned probabilities beyond the first n heads (trainer, per step)
@@ -1061,8 +1063,26 @@ class AttentionTCFn(torch.autograd.Function):
         return dq_buf, (None if same else dkv_buf), dpe, None, None
 
 
+def attention_decode(q_buf, kv_buf, *, H, d, q_col, k_col, v_col, scale, key_pad=None, return_probs=False):
+    """One query row per utterance (incremental decoding, forward only) on st5_attn_decode_fwd: q_buf [B, 1, nq*d],
+    kv_buf [B, Tk, nk*d] with q / k / v in column blocks q_col / k_col / v_col (kv_buf None: q_buf), key_pad [B, Tk]
+    (nonzero / True = masked). Returns (out [B, 1, d], probs [B, H, 1, Tk] fp32 when return_probs else None)."""
+    kvb = q_buf if kv_buf is None else kv_buf
+    B, Tk = kvb.shape[0], kvb.shape[1]
+    assert q_buf.shape[1] == 1 and d == H * 64 and q_buf.dtype == kvb.dtype
+    out = torch.empty((B, 1, d), dtype=q_buf.dtype, device=q_buf.device)
+    probs = torch.empty((B, H, 1, Tk), dtype=torch.float32, device=q_buf.device) if return_probs else None
+    K.attn_decode_fwd(q_buf.narrow(2, q_col * d, d), kvb.narrow(2, k_col * d, d), kvb.narrow(2, v_col * d, d), out,
+                      H=H, scale=scale, key_pad=_key_pad_u8(key_pad), probs=probs)
+    return out, probs
+
+
 def attention(q_buf, kv_buf, *, H, d, q_col, k_col, v_col, scale, pe_k=None, maxpos=0, key_pad=None, causal=False,
               drop_p=0.0, return_probs=False):
+    if RT.attn_decode_rows and q_buf.shape[1] == 1 and pe_k is None and not causal and drop_p == 0.0 \
+            and not torch.is_grad_enabled():
+        return attention_decode(q_buf, kv_buf, H=H, d=d, q_col=q_col, k_col=k_col, v_col=v_col, scale=scale,
+                                key_pad=key_pad, return_probs=return_probs)
     # RT.probs_grad_heads: the consumer of the returned probabilities differentiates only through the first n heads (the
     # guided-attention loss; set by the trainer from the criterion): the backward skips the zero gradient of the others
     cfg = dict(H=H, d=d, q_col=q_col, k_col=k_col, v_col=v_col, scale=scale, maxpos=maxpos, causal=causal,

@@ -121,6 +121,15 @@ class SpeechT5Task(LegacyFairseqTask):
             encoder_input.update(kwargs)
             return models[0].generate_speech(**encoder_input)
 
+    def generate_speech_batch(self, models, net_input, **kwargs):
+        """generate_speech for every utterance of a collated t2s (src_tokens, src_lengths, spkembs) or s2s (source,
+        padding_mask, spkembs) net_input in one batched decode; each utterance's padding is stripped first. Returns
+        models[0].generate_speech_batch's list of (mel, stop probabilities, attention or None)."""
+        keys = ("source", "padding_mask") if "source" in net_input else ("src_tokens", "src_lengths")
+        args = {k: net_input.get(k) for k in keys + ("spkembs",)}
+        args.update(kwargs)
+        return models[0].generate_speech_batch(**args)
+
     def generate_class(self, models, net_input, prefix_tokens, **kwargs):
         """tasks/speecht5.py:631-638 (what scripts/generate_class.py calls): the predicted class of every utterance."""
         with torch.no_grad():
