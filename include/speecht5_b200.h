@@ -147,7 +147,11 @@ int st5_colsum(const void* x, int64_t ld, float* out, int dtype, int64_t rows, i
  * scores = scale * q.(k + pe_k[clamp(i-j,-maxpos,maxpos-1)+maxpos]) (RPE, encoder.py:40-59,239-246) ;
  * causal => j <= i; key_pad[b][j] != 0 => -inf; P = softmax_fp32; out = dropout(P) v.
  * probs (optional) receives P: [B,H,Tq,p_ld] in `probs_dtype` (fp32 when returned to the user: need_head_weights).
- * Head dim is fixed at 64 (Base and Large). */
+ * Head dim is fixed at 64 (Base and Large).
+ * A query row whose keys are all masked is produced by no caller; the entry points differ there: st5_attn_fwd returns
+ * NaN for it (softmax of an all -inf row, as the reference does), st5_attn_fused_fwd / st5_attn_flash_fwd return zeros
+ * (inv_l = 0, lse = -inf). Keys no query row sees (masked, or j >= Tq under the causal mask) get exactly zero dK / dV.
+ * dprobs_ext: only columns j < Tk are read (the padding columns [Tk, p_ld) may hold anything). */
 typedef struct st5_attn_args {
   int32_t B, H, Tq, Tk, dtype, causal, maxpos, probs_dtype;
   const void* q; int64_t q_ld, q_bs;
@@ -199,11 +203,14 @@ int st5_attn_decode_fwd(const st5_attn_decode_args* args, void* stream);
 
 /* Fused wgmma attention forward (bf16, Tk <= 320): QK^T -> masks -> softmax -> dropout -> PV in ONE launch, no score
  * or probability round trip through HBM. Uses the q/k/v/out/probs/key_pad/scale/dropout fields of st5_attn_args exactly
- * like st5_attn_fwd; additionally writes lse[b][h][i] = log sum_j exp(scale*q_i.k_j) (may be NULL). probs (optional,
+ * like st5_attn_fwd; additionally writes lse[b][h][i] = log sum_j exp(s_ij) over the keys row i sees (natural log, the
+ * masked scores s of the contract above; may be NULL -- no caller passes it today). probs (optional,
  * only when the caller wants them: need_head_weights) receives the undropped normalised probabilities in probs_dtype.
  * What the backward pass reads back (both optional, but together): psave [B,H,Tq,p_ld] BF16 = exp(s - rowmax), NOT
  * normalised, with the SIGN BIT set on elements dropout removed (probabilities are non-negative; a dropped zero is -0),
- * and inv_l [B,H,Tq] = 1 / rowsum. p_ld must be a multiple of 8, psave 16-byte aligned. out_f32 (optional)
+ * and inv_l [B,H,Tq] = 1 / rowsum. p_ld must be a multiple of 8, psave 16-byte aligned. psave holds zeros on every
+ * masked key and in the columns [Tk, p_ld) of every key block the backward reads (under the causal mask: the blocks up
+ * to the row's own 64-row tile; later blocks are neither written nor read). out_f32 (optional)
  * [B,Tq,H*64] FP32 receives the un-rounded output: the backward's row constant delta = dO.O is the subtrahend of a
  * cancelling difference (dS = P (dP - delta)) and must not carry the BF16 rounding of `out`.
  * Relative positions (encoder.py:239-246): pe_k != NULL selects the skewed-bias variant; here pe_k must point to a
@@ -223,7 +230,8 @@ int st5_attn_flash_fwd(const st5_attn_args* args, float* lse, void* psave, float
  * args->probs must be the FP32 probabilities the forward returned); writes dq/dk/dv (same layouts as q/k/v).
  * ext_heads > 0: dprobs_ext is known to be zero for heads >= ext_heads (the guided-attention loss reads the first two
  * heads of every layer, text_to_speech_loss.py:210-212) -- those heads skip its loads. out_f32 (optional): what the
- * forward wrote there. Scratch: delta [B*H*Tq] floats, dq_acc [B*Tq*H*64] floats.
+ * forward wrote there. Scratch: delta [B*H*Tq] floats, dq_acc [B*Tq*H*64] floats (any contents: written before read).
+ * dprobs_ext: columns [Tk, p_ld) and heads >= ext_heads (when 0 < ext_heads < H) are never read.
  * Relative positions (pe_k != NULL): args->ds additionally receives dS as BF16 [B,H,Tq,p_ld] for st5_attn_dqp_scatter
  * and the two table GEMMs; dq then holds only the q.k part of the gradient. */
 int st5_attn_fused_bwd(const st5_attn_args* args, const void* psave, const float* inv_l, const float* out_f32,

@@ -203,7 +203,17 @@ __global__ void __launch_bounds__(FB_THREADS, 1)
     int it = 0, kbc = 0;
     for (int kb = 0; kb < nkb; ++kb) {
       const int qt0 = p.causal ? kb : 0;
-      if (qt0 >= nqt) continue;
+      if (qt0 >= nqt) {  // causal, Tk > Tq: no query row sees the keys of this block, their gradients are zero
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+          const int key = kb * FB_T + r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
+          if (key < p.Tk) {
+            *reinterpret_cast<uint32_t*>(p.dk + (int64_t)b * p.k_bs + (int64_t)key * p.k_ld + h * 64 + col) = 0u;
+            *reinterpret_cast<uint32_t*>(p.dv + (int64_t)b * p.v_bs + (int64_t)key * p.v_ld + h * 64 + col) = 0u;
+          }
+        }
+        continue;
+      }
       mbar_wait_quiet(bar_kv, (uint32_t)(kbc & 1));
       ++kbc;
       for (int qt = qt0; qt < nqt; ++qt, ++it) {
@@ -338,14 +348,13 @@ __global__ void __launch_bounds__(FB_THREADS, 1)
           const uint32_t w4[4] = {praw.x, praw.y, praw.z, praw.w};
           float xd[8];
           xd[0] = xd[1] = xd[2] = xd[3] = xd[4] = xd[5] = xd[6] = xd[7] = 0.f;
-          if (dpx != nullptr) {  // the caller's gradient on the probabilities: this row's 8 floats of the chunk
-            if ((p.p_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(p.dp_ext) & 15) == 0) {
-              if (col0 + 8 * g + 8 <= p.p_ld) {
-                const float4 x0 = __ldg(reinterpret_cast<const float4*>(dpx + col0 + 8 * g));
-                const float4 x1 = __ldg(reinterpret_cast<const float4*>(dpx + col0 + 8 * g + 4));
-                xd[0] = x0.x; xd[1] = x0.y; xd[2] = x0.z; xd[3] = x0.w;
-                xd[4] = x1.x; xd[5] = x1.y; xd[6] = x1.z; xd[7] = x1.w;
-              }
+          if (dpx != nullptr) {  // the caller's gradient on the probabilities: this row's 8 floats of the chunk (keys
+                                 // < Tk only: the padding columns [Tk, p_ld) are not part of the contract)
+            if ((p.p_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(p.dp_ext) & 15) == 0 && col0 + 8 * g + 8 <= p.Tk) {
+              const float4 x0 = __ldg(reinterpret_cast<const float4*>(dpx + col0 + 8 * g));
+              const float4 x1 = __ldg(reinterpret_cast<const float4*>(dpx + col0 + 8 * g + 4));
+              xd[0] = x0.x; xd[1] = x0.y; xd[2] = x0.z; xd[3] = x0.w;
+              xd[4] = x1.x; xd[5] = x1.y; xd[6] = x1.z; xd[7] = x1.w;
             } else {
 #pragma unroll
               for (int t = 0; t < 8; ++t)
