@@ -30,9 +30,15 @@ extern "C" {
 #define ST5_BF16 1
 #define ST5_ACT_NONE 0
 #define ST5_ACT_RELU 1
-#define ST5_ACT_GELU 2
+#define ST5_ACT_GELU 2      /* x Phi(x), Phi from the Abramowitz-Stegun 7.1.26 erf (|error| <= 1.5e-7 in erf) with
+                               approximate rcp / ex2: |error| <= 2.5e-7 |x| + a few fp32 ulps of the result */
 #define ST5_ACT_TANH 3
-#define ST5_ACT_GELU_TANH 4 /* tanh-form GELU on the MUFU unit: |error| <= 4.8e-4 vs the erf form; bf16 throughput mode */
+#define ST5_ACT_GELU_TANH 4 /* tanh-form GELU on the MUFU unit: |error| <= 4.8e-4 vs the erf form (4.74e-4 measured over
+                               every bf16 input, at x = 2.7; below half a bf16 ulp of the result wherever |y| > 0.13);
+                               bf16 throughput mode */
+/* Non-finite inputs of st5_act_fwd / st5_act_bwd: RELU maps NaN to 0 (fmaxf) and its derivative is 0 at NaN and x <= 0;
+ * TANH gives +-1 at +-inf, derivative 0; GELU / GELU_TANH give +inf at +inf and NaN at -inf and NaN, and their
+ * derivatives NaN at +-inf and NaN (GELU_TANH's also for finite |x| >= 2^64, where x * x overflows). */
 #define ST5_ACT_GATE 5      /* actgrad_act only: actgrad_pre already holds the multiplier (written by ..._GATE below) */
 #define ST5_ACT_GELU_TANH_GATE 6 /* act only (bf16 output, N % 8 == 0, c_pre != NULL): C = dropout(gelu_tanh(x)) and c_pre
                                     receives keep * scale * gelu_tanh'(x), the factor of the FFN's dH GEMM in backward */
@@ -78,13 +84,14 @@ typedef struct st5_gemm_args {
 } st5_gemm_args;
 int st5_gemm_bf16(const st5_gemm_args* args, void* stream);
 
-/* fp32 -> bf16 cast of a strided 2-D view. lo != NULL additionally writes the bf16 residual x - float(hi(x)), which
+/* fp32 -> bf16 cast of a strided 2-D view: hi = round-to-nearest-even(x). lo != NULL additionally writes the bf16
+ * residual round-to-nearest-even(x - float(hi(x))), which
  * lets callers form hi*hi + hi*lo + lo*hi with three accumulate passes of st5_gemm_bf16 (fp32-grade "parity mode"). */
 int st5_cast_bf16(const float* src, int64_t src_ld, void* hi, void* lo, int64_t dst_ld, int64_t rows, int64_t cols,
                   void* stream);
 
 /* ------------------------------------------------------------------------------------------------- pre-nets
- * y[b,t,:] = dropout( (tokens ? E[tokens[b,t]] : x[b,t,:]) + alpha * pe[t,:] ).
+ * y[b,t,:] = dropout( (tokens ? E[tokens[b,t]] : x[b,t,:]) + alpha * pe[t,:] ); pe has at least T rows of C floats.
  * text_encoder_prenet.py:36-45 (Embedding -> espnet ScaledPositionalEncoding), speech_decoder_prenet.py:52-67. */
 int st5_posenc_fwd(const int64_t* tokens, const float* emb, const void* x, const float* pe, const float* alpha,
                    void* y, int dtype, int64_t B, int64_t T, int64_t C, float drop_p, uint64_t seed, uint64_t offset,
@@ -95,7 +102,10 @@ int st5_posenc_bwd(const void* dy, const int64_t* tokens, int64_t padding_idx, c
                    uint64_t offset, void* stream);
 
 /* ------------------------------------------------------------------------------------------------- LayerNorm
- * s = residual + dropout(x); y = LN(s) * gamma + beta. Saves s (for backward), mean and rstd.
+ * s = residual + dropout(x); y = LN(s) * gamma + beta (biased variance, eps inside the square root). Saves s (for
+ * backward), mean and rstd (each may be NULL). C % 8 == 0 and 0 < C <= 1024; every row tensor and gamma / beta are read
+ * and written as 16-byte vectors, so their base pointers must be 16-byte aligned (mean / rstd / dgamma / dbeta / dxsum
+ * need only float alignment). Anything else returns -2 before any launch.
  * transformer_layer.py:112-132 (post-LN encoder layer), :343-391 (decoder layer), encoder.py:226-227. */
 int st5_ln_fwd(const void* x, const void* residual, const float* gamma, const float* beta, void* y, void* s_out,
                float* mean, float* rstd, int dtype, int64_t rows, int64_t C, float eps, float drop_p, uint64_t seed,
@@ -255,8 +265,14 @@ int st5_attn_dqp_scatter(const void* ds_bf16, void* dqp_bf16, int32_t B, int32_t
                          int64_t p_ld, int32_t maxpos, int32_t h_major, void* stream);
 
 /* ------------------------------------------------------------------------------------------------- BatchNorm1d
- * espnet Tacotron2 Postnet block (speech_decoder_postnet.py:39-51): y = dropout(tanh?(BN(x))) on channels-last
- * rows [rows][C]; training statistics over all rows (padded frames included, as in the reference). */
+ * espnet Tacotron2 Postnet block (speech_decoder_postnet.py:39-51): y = dropout(act(BN(x))) on channels-last
+ * rows [rows][C] (row pitches x_ld, y_ld, dy_ld, dx_ld); training statistics over all rows (padded frames included, as
+ * in the reference): save_mean / save_rstd from the biased variance (eps inside the square root), running_var updated
+ * with the unbiased one. rows == 1 (torch refuses it) uses var = 0 and moves running_var towards that biased 0.
+ * Eval (training == 0): save_mean / save_rstd are derived from the running statistics, which are only read.
+ * y_pre (optional in forward, required by the backward when act != ST5_ACT_NONE, else it returns -2) is contiguous
+ * [rows][C]: the value before act(). Dropout index = row * C + c. act: NONE, RELU or TANH. scratch: 2 * C floats (any
+ * contents). Backward: dgamma / dbeta are accumulated (+=). */
 int st5_bn_fwd(const void* x, int64_t x_ld, const float* gamma, const float* beta, float* running_mean,
                float* running_var, float* save_mean, float* save_rstd, void* y, int64_t y_ld, void* y_pre, int dtype,
                int64_t rows, int64_t C, int training, float momentum, float eps, int act, float drop_p, uint64_t seed,
@@ -384,8 +400,12 @@ int st5_time_mean_bwd(const void* dy, void* dx, int dtype, int64_t B, int64_t T,
  * gradient scale (grad_mul x clip coefficient max_norm / (norm + 1e-6) capped at 1: fairseq/utils.py clip_grad_norm_,
  * fairseq/trainer.py:796-826), Adam as fairseq/optim/adam.py:Adam.step writes it (denominator sqrt(v) + eps, step size
  * lr * sqrt(1 - b2^t) / (1 - b1^t), weight decay p -= wd * lr * p) and refreshes the bf16 shadow copy the GEMMs read.
- * st5_sumsq accumulates sum(x^2) (the squared gradient norm) into *out. lr_dev / step_dev: device-resident schedule
- * state so that a captured CUDA graph stays valid across updates. */
+ * The clip norm is that of the grad_mul-scaled gradient: sqrt(*grad_norm_sq) * grad_mul (no clip when max_norm <= 0 or
+ * grad_norm_sq is NULL). When *grad_norm_sq is NaN, inf or above 3e38 the launch changes nothing (p, m, v, shadow).
+ * st5_sumsq accumulates sum(x^2) (the squared gradient norm) into *out; x must be 16-byte aligned (else -2).
+ * lr_dev / step_dev: device-resident schedule state so that a captured CUDA graph stays valid across updates. lr_dev
+ * replaces `lr` everywhere (also in the weight decay); step_dev replaces `step` (then `step` is not read, else it must
+ * be >= 1: -2). p_bf16 may be NULL; p, g, m, v 16-byte aligned and p_bf16 8-byte aligned take the vector path. */
 int st5_sumsq(const float* x, int64_t n, float* out /* 1 float, accumulated */, void* stream);
 int st5_adam_step(float* p, const float* g, float* m, float* v, void* p_bf16, int64_t n, float lr, float beta1,
                   float beta2, float eps, float weight_decay, int64_t step, const float* grad_norm_sq, float max_norm,

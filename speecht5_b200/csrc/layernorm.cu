@@ -6,6 +6,7 @@
 //   backward: ds = rstd * (g - mean(g) - xhat * mean(g * xhat)),  g = dy * gamma ;  dx = dropout_bwd(ds)
 //             dgamma += sum_rows dy * xhat ; dbeta += sum_rows dy     (separate column-reduction kernel)
 #include "kernels.cuh"
+#include <initializer_list>
 #include <stdlib.h>
 #include "ptx.cuh"
 #include "vec8.cuh"
@@ -90,11 +91,20 @@ __global__ void __launch_bounds__(LN_WARPS * 32)
   }
 }
 
+// Every row tensor and gamma / beta are accessed as 16-byte vectors: with C % 8 == 0 each row is aligned when its base
+// is, so a misaligned base (an offset view) is rejected here instead of faulting in the kernel. NULL passes.
+static bool ln_aligned(std::initializer_list<const void*> ptrs) {
+  for (const void* q : ptrs)
+    if (reinterpret_cast<uintptr_t>(q) & 15) return false;
+  return true;
+}
+
 int ln_fwd_launch(const void* x, const void* residual, const float* residual_f32, const float* gamma, const float* beta,
                   void* y, float* y_f32, void* s_out, float* mean, float* rstd, int dtype, int64_t rows, int64_t C,
                   float eps, float drop_p, uint64_t seed, uint64_t offset, cudaStream_t s) {
   if (rows == 0) return 0;
   if (C > 8 * 32 * LN_MAX_CHUNKS || C <= 0 || (C & 7)) return -2;
+  if (!ln_aligned({x, residual, residual_f32, gamma, beta, y, y_f32, s_out})) return -2;
   const uint32_t thr = drop_threshold(drop_p);
   const float ds = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
   const unsigned grid = (unsigned)((rows + LN_WARPS - 1) / LN_WARPS);
@@ -418,6 +428,7 @@ int ln_bwd_launch(const void* dy, const void* s_in, const float* mean, const flo
                   float drop_p, uint64_t seed, uint64_t offset, cudaStream_t s) {
   if (rows == 0) return 0;
   if (C > 8 * 32 * LN_MAX_CHUNKS || C <= 0 || (C & 7)) return -2;
+  if (!ln_aligned({dy, s_in, gamma, ds, dx})) return -2;  // (dgamma / dbeta / dxsum: any float alignment)
   const uint32_t thr = drop_threshold(drop_p);
   const float dsc = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
   if ((dgamma != nullptr || dbeta != nullptr || dxsum != nullptr) && (rows >= 64 || dxsum != nullptr)) {
