@@ -322,7 +322,10 @@ int st5_conv0_ln_gelu_bwd(const void* dy, const float* wave, const float* w, con
  * an infeasible utterance, or 0 with zero_infinity); grad (optional, same addressing as logits) receives
  * d(sum_b nll_b)/d logits, zero for t >= input_lengths[b] and for infeasible utterances. S_max >= 2*max(target_lengths)+1
  * (<= 1024) is the scratch pitch; ws: st5_ctc_ws_floats(T, B, S_max) floats (row log-sum-exps, emission terms, alpha
- * and beta lattices). Three launches: row pass, the two recursions side by side in one CTA per utterance, gradient rows. */
+ * and beta lattices). Three launches: row pass, the two recursions side by side in one CTA per utterance, gradient rows.
+ * Utterances with input_lengths[b] <= 0 or 2*target_lengths[b]+1 > S_max are reported infeasible; rows t >= T are never
+ * read (input_lengths > T counts as T). With grad != NULL, V <= 12288 (the gradient's per-symbol sums of a row live in
+ * 48 KiB of shared memory), else -2 before any launch. */
 int64_t st5_ctc_ws_floats(int32_t T, int32_t B, int32_t S_max);
 int st5_ctc_loss(const float* logits, int64_t ld_t, int64_t ld_b, const int64_t* targets, const int64_t* tgt_offsets,
                  const int64_t* input_lengths, const int64_t* target_lengths, float* nll, float* grad, float* ws,
@@ -337,7 +340,9 @@ int st5_ctc_loss(const float* logits, int64_t ld_t, int64_t ld_b, const int64_t*
  * sums: scratch of st5_tts_loss_ws_floats(B, L) floats that st5_tts_loss_bwd reads back (sums[3] = number of valid
  * frames; the rest holds per-CTA partials, added in a fixed order: same inputs, same bits).
  * st5_tts_loss_bwd (gradient of text_to_speech_loss.py:288-330): g[3] = upstream gradients of (l1, l2, bce) in device memory; writes d_after, d_before [B, L, D] and
- * d_logits [B, L] everywhere (zeros outside the masks). */
+ * d_logits [B, L] everywhere (zeros outside the masks); sign(0) = 0 in the L1 gradient.
+ * D % 4 == 0 selects 16-byte vector accesses: then after, before, ys (and d_after, d_before) must be 16-byte aligned
+ * and y_bs a multiple of 4, else -2 before any launch. */
 int64_t st5_tts_loss_ws_floats(int32_t B, int32_t L);
 int64_t st5_guided_attn_ws_floats(int32_t n_layers, int32_t B, int32_t heads, int32_t T_out);
 int st5_tts_loss_fwd(const float* after, const float* before, const float* logits, const float* ys, int64_t y_bs,
@@ -349,7 +354,9 @@ int st5_tts_loss_bwd(const float* after, const float* before, const float* logit
                      float* d_logits, void* stream);
 /* GuidedMultiHeadAttentionLoss (text_to_speech_loss.py:370-427) over the first `heads` heads of n_layers (<= 8) returned cross-attention
  * probability tensors att[i] = [B, H, T_out, p_ld] fp32: out[0] = alpha * sum_valid W * A / (sum_b il_b * ol_b * heads *
- * n_layers), W = 1 - exp(-(t_in / il - t_out / ol)^2 / (2 sigma^2)), ol = olens[b] / r, il = ilens[b]. gsum: scratch of
+ * n_layers), W = 1 - exp(-(t_in / il - t_out / ol)^2 / (2 sigma^2)), ol = olens[b] / r, il = ilens[b]. The valid region
+ * (t_out < min(T_out, ol), t_in < min(T_in, il)) and the normaliser take the clamped lengths; W divides by the unclamped
+ * il and ol. gsum: scratch of
  * st5_guided_attn_ws_floats(n_layers, B, heads, T_out) floats (fixed-order partial sums)
  * read back by the backward, which writes datt[i] (same layout) = g[0] * d out / d att on heads < `heads`; the other
  * heads are cleared only with zero_rest != 0 (st5_attn_fused_bwd with ext_heads never reads them). */
@@ -378,10 +385,12 @@ int st5_l2norm_rows_bwd(const float* dy, const float* y, const float* nrm, void*
  * x > 0 else x, speaker_decoder_postnet.py:118-126) and every other column s x. z_out (optional, pitch z_ld) receives z.
  * With target != NULL: log-softmax of z, then per row stats[4 b + 0..3] = label-smoothed loss (weights 1 - eps - eps_i
  * on the target, eps_i = eps / (N - 1) on every class), nll, arg-max correct (lowest index among equal maxima), valid;
- * all 0 on a row whose target is ignore_index. lse [B] is saved for the backward.
+ * all 0 on a row whose target is ignore_index; a target outside [0, N) (and not ignore_index) gives NaN loss and nll.
+ * lse [B] is saved for the backward.
  * st5_margin_ce_bwd: d z from the loss (target != NULL: gstat[0] d loss + gstat[1] d nll per valid row, both device
  * floats) or given (dz_in, pitch dz_ld); dx [B, N] fp32 (pitch dx_ld) = d z . d z / d x, including d phi / d x on the
- * margin column. Same margin arguments as the forward. */
+ * margin column (AAM: d sine / d x = -x / sine, taken as 0 where sine = 0, i.e. at |x| >= 1). Same margin arguments as
+ * the forward. */
 int st5_margin_ce_fwd(const float* x, int64_t x_ld, int32_t B, int32_t N, const int64_t* mtarget, int mode, float scale,
                       float margin, int easy_margin, float* z_out, int64_t z_ld, const int64_t* target, float eps,
                       int64_t ignore_index, float* stats, float* lse, void* stream);

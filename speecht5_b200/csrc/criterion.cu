@@ -9,6 +9,7 @@
 //       layers' returned cross-attention probabilities, ol = olens / r (decoder steps), il = text length.
 // HBM-bound passes: forward reads after, before, y once (3 x B*L*odim fp32) -- warp per frame row, 16-byte loads.
 #include "kernels.cuh"
+#include <initializer_list>
 #include <math_constants.h>
 
 namespace st5 {
@@ -262,6 +263,16 @@ __global__ void __launch_bounds__(CR_WARPS * 32)
 }
 
 int64_t tts_loss_blocks(int B, int L) { return ((int64_t)B * L + CR_WARPS - 1) / CR_WARPS; }
+
+// D % 4 == 0 selects the float4 path, which needs every [B, L, D] operand 16-byte aligned and the ys batch pitch a
+// multiple of 4; a misaligned call is rejected before any launch instead of faulting in the kernel. NULL passes.
+static bool tts_vec_ok(int D, int64_t y_bs, std::initializer_list<const void*> ptrs) {
+  if (D & 3) return true;
+  if (y_bs & 3) return false;
+  for (const void* q : ptrs)
+    if (reinterpret_cast<uintptr_t>(q) & 15) return false;
+  return true;
+}
 int64_t guided_attn_blocks(int n_layers, int B, int heads, int T_out) {
   return ((int64_t)n_layers * B * heads * T_out + CR_WARPS - 1) / CR_WARPS;
 }
@@ -269,7 +280,7 @@ int64_t guided_attn_blocks(int n_layers, int B, int heads, int T_out) {
 int tts_loss_fwd_launch(const float* after, const float* before, const float* logits, const float* ys, int64_t y_bs,
                         const float* labels, int64_t lab_bs, const int64_t* olens, int B, int L, int D, int r,
                         float pos_weight, float* sums, float* out, cudaStream_t s) {
-  if (B <= 0 || L <= 0 || D <= 0 || r <= 0) return -2;
+  if (B <= 0 || L <= 0 || D <= 0 || r <= 0 || !tts_vec_ok(D, y_bs, {after, before, ys})) return -2;
   const int64_t nblk = tts_loss_blocks(B, L);
   launch_pdl(tts_loss_fwd_kernel, dim3((unsigned)nblk), dim3(CR_WARPS * 32), 0, s, after, before, logits, ys, y_bs, labels, lab_bs, olens, B, L, D, r, pos_weight, sums);
   launch_pdl(tts_loss_finalize_kernel, dim3(1), dim3(256), 0, s, sums, nblk, D, out);
@@ -280,7 +291,7 @@ int tts_loss_bwd_launch(const float* after, const float* before, const float* lo
                         const float* labels, int64_t lab_bs, const int64_t* olens, const float* sums, const float* g,
                         int B, int L, int D, int r, float pos_weight, float* d_after, float* d_before, float* d_logits,
                         cudaStream_t s) {
-  if (B <= 0 || L <= 0 || D <= 0 || r <= 0) return -2;
+  if (B <= 0 || L <= 0 || D <= 0 || r <= 0 || !tts_vec_ok(D, y_bs, {after, before, ys, d_after, d_before})) return -2;
   const int64_t rows = (int64_t)B * L;
   launch_pdl(tts_loss_bwd_kernel, dim3((unsigned)((rows + CR_WARPS - 1) / CR_WARPS)), dim3(CR_WARPS * 32), 0, s, after, before, logits, ys, y_bs, labels, lab_bs, olens, sums, g, B, L, D, r, pos_weight, d_after, d_before, d_logits);
   return (int)cudaGetLastError();

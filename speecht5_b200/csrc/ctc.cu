@@ -189,6 +189,11 @@ int ctc_loss_launch(const float* logits, int64_t ld_t, int64_t ld_b, const int64
                     int32_t T, int32_t B, int32_t V, int32_t S_max, int32_t blank, int32_t zero_infinity,
                     cudaStream_t st) {
   if (T <= 0 || B <= 0 || V <= 0 || S_max <= 0 || S_max > 1024 || blank < 0 || blank >= V) return -2;
+  // the gradient kernel keeps one fp32 row of V per-symbol sums per warp in 48 KiB of shared memory; checked before any
+  // launch so that a rejected call writes nothing
+  int warps = CTC_ROW_WARPS;
+  while (warps > 1 && (size_t)warps * V * sizeof(float) > 48 * 1024) warps >>= 1;
+  if (grad != nullptr && (size_t)warps * V * sizeof(float) > 48 * 1024) return -2;
   float* lse = ws;
   float* nll_raw = ws + (int64_t)T * B;
   float* lp = nll_raw + B;
@@ -203,9 +208,6 @@ int ctc_loss_launch(const float* logits, int64_t ld_t, int64_t ld_b, const int64
                                                                        target_lengths, nll, nll_raw, alpha, beta, T, S_max,
                                                                        SP, blank, zero_infinity);
   if (grad != nullptr) {
-    int warps = CTC_ROW_WARPS;
-    while (warps > 1 && (size_t)warps * V * sizeof(float) > 48 * 1024) warps >>= 1;
-    if ((size_t)warps * V * sizeof(float) > 48 * 1024) return -5;
     ctc_grad_kernel<<<(rows + warps - 1) / warps, warps * 32, (size_t)warps * V * sizeof(float), st>>>(
         logits, ld_t, ld_b, lse, lp, alpha, beta, nll_raw, targets, tgt_offsets, input_lengths, target_lengths, grad, T, B,
         V, S_max, blank, warps);
