@@ -196,7 +196,9 @@ int st5_attn_bwd(const st5_attn_args* args, void* stream);
  * Keys are reduced in fixed splits of 64 (split-KV over grid (splits, H, B), merged by a second launch when Tk > 64):
  * a masked key adds an exact zero, so an utterance's result is bit-identical at any B and any key span Tk that holds
  * its valid keys. ws: st5_attn_decode_ws_floats(B, H, Tk, probs != NULL) floats of scratch (none for Tk <= 64).
- * K / V rows and strides must be 16-byte aligned. */
+ * An utterance whose keys are all masked is produced by no caller; its output and probabilities are zeros (at any Tk).
+ * Returns -2 for B, H or Tk <= 0, -5 for ws == NULL with Tk > 64, and -6 unless k, v, k_ld, v_ld, k_bs and v_bs are
+ * 16-byte aligned (pointers, and strides in bytes); nothing is written then. */
 typedef struct st5_attn_decode_args {
   int32_t B, H, Tk, dtype;
   const void* q; int64_t q_bs;
@@ -289,8 +291,12 @@ int st5_bn_bwd(const void* dy, int64_t dy_ld, const void* x, int64_t x_ld, const
  * (fairseq/modules/gelu.py:24), fused. wave [B, n_samples] fp32; w [C, K]; y [B, T0, C] channels-last in `dtype`,
  * T0 = (n_samples - K) / stride + 1; mean / rstd [B, C] are saved for the backward. The convolution is recomputed from
  * the waveform in every pass, so the [B, T0, C] tensor is written once (forward) and dy read twice (backward).
- * ws: st5_conv0_ws_floats(...) floats of scratch. act: ST5_ACT_GELU or ST5_ACT_GELU_TANH. C <= 1024, K <= 16.
- * Backward: dw [C, K], dgamma [C], dbeta [C] are ACCUMULATED (+=); the input is the waveform: no input gradient. */
+ * Samples past (T0 - 1) * stride + K of each row are not read. ws: st5_conv0_ws_floats(...) floats of scratch (any
+ * contents). act: ST5_ACT_GELU or ST5_ACT_GELU_TANH. GroupNorm: biased variance over the T0 frames, eps inside the
+ * square root (a constant channel gets rstd = eps^-1/2). Backward: dw [C, K], dgamma [C], dbeta [C] are ACCUMULATED
+ * (+=); the input is the waveform: no input gradient. Returns, with nothing written: -2 unless B >= 1, 1 <= C <= 1024,
+ * 1 <= K <= 16 and stride >= 1; -3 for another act; -4 when T0 < 1 (n_samples < K); -5 when a block's waveform segment,
+ * (127 * stride + K) floats, exceeds 48 KiB (stride > 96). */
 int64_t st5_conv0_ws_floats(int32_t B, int64_t n_samples, int32_t C, int32_t K, int32_t stride);
 int st5_conv0_gn_gelu_fwd(const float* wave, const float* w, const float* gamma, const float* beta, void* y, int dtype,
                           float* mean, float* rstd, float* ws, int32_t B, int64_t n_samples, int32_t C, int32_t K,
@@ -304,7 +310,9 @@ int st5_conv0_gn_gelu_bwd(const void* dy, const float* wave, const float* w, con
  * speech_encoder_prenet.py:308-318): Conv1d(1 -> C, K taps, `stride`, no bias) + Fp32LayerNorm over the C channels of
  * each frame + GELU, fused in ONE pass (a warp per frame). y [B, T0, C] channels-last in `dtype`; mean / rstd [B * T0]
  * are saved for the backward. C even, C <= 512, K <= 16. Backward: dw [C, K], dgamma [C], dbeta [C] are ACCUMULATED
- * (+=); ws: st5_conv0_ln_ws_floats(...) floats of scratch; no input gradient (the input is the waveform). */
+ * (+=); ws: st5_conv0_ln_ws_floats(...) floats of scratch (any contents); no input gradient (the input is the
+ * waveform). Returns, with nothing written: -2 unless B >= 1, C even in [2, 512], 1 <= K <= 16 and stride >= 1; -3 for
+ * another act; -4 when T0 < 1. No stride limit. */
 int64_t st5_conv0_ln_ws_floats(int32_t B, int64_t n_samples, int32_t C, int32_t K, int32_t stride);
 int st5_conv0_ln_gelu_fwd(const float* wave, const float* w, const float* gamma, const float* beta, void* y, int dtype,
                           float* mean, float* rstd, int32_t B, int64_t n_samples, int32_t C, int32_t K, int32_t stride,

@@ -8,7 +8,8 @@
 // split to (max, sum of exponentials, 64-wide unnormalised accumulator); a combine kernel merges the splits in index
 // order. Key j always lands in split j / DCH at the same lane position, and a masked key adds an exact zero (a split
 // whose keys are all masked merges with weight zero), so an utterance's result depends only on its own valid keys: not
-// on B and not on the buffer's key span (the bucket of a captured graph).
+// on B and not on the buffer's key span (the bucket of a captured graph). An utterance whose keys are all masked has
+// l = 0 on both paths; 1 / l is then taken as 0, so its output and probabilities are zeros on both paths alike.
 #include "kernels.cuh"
 
 namespace st5 {
@@ -131,7 +132,7 @@ __global__ void __launch_bounds__(DT) attn_decode_split(const st5_attn_decode_ar
 #pragma unroll
     for (int w = 1; w < DT / 32; ++w) r += part[w][tid];
     if (direct) {
-      stf((T*)a.out + (int64_t)b * a.o_bs + h * DH + tid, r * (1.f / l));
+      stf((T*)a.out + (int64_t)b * a.o_bs + h * DH + tid, r * (l > 0.f ? 1.f / l : 0.f));
     } else {
       float* pr = a.ws + (bh * n_splits + s) * DPART;
       pr[2 + tid] = r;
@@ -141,7 +142,7 @@ __global__ void __launch_bounds__(DT) attn_decode_split(const st5_attn_decode_ar
   if (direct) {
     float* pr = decode_probs(a, b, h);
     if (pr != nullptr) {
-      const float inv = 1.f / l;
+      const float inv = l > 0.f ? 1.f / l : 0.f;
       for (int j = tid; j < a.Tk; j += DT) pr[j] = sc[j] * inv;
     }
   }
@@ -159,7 +160,7 @@ __global__ void __launch_bounds__(DT) attn_decode_combine(const st5_attn_decode_
     const float ms = pr[s * DPART];
     L += ms == -INFINITY ? 0.f : pr[s * DPART + 1] * expf(ms - M);
   }
-  const float inv = 1.f / L;
+  const float inv = L > 0.f ? 1.f / L : 0.f;
   if (tid < DH) {
     float r = 0.f;
     for (int s = 0; s < ns; ++s) {

@@ -8,7 +8,9 @@
 //   forward : pass 1 statistics (reads the waveform only), pass 2 normalise + GELU + store  -> 1 write of [B, T, C]
 //   backward: pass 1 sums of g and g*xhat (reads dy), pass 2 weight gradient (reads dy)      -> 2 reads of [B, T, C]
 // The input is the waveform, so there is no input gradient. One thread per channel, TCH output frames per block, the
-// waveform segment of the block staged in shared memory (every thread reads the same address: broadcast).
+// waveform segment of the block staged in shared memory (every thread reads the same address: broadcast). A block holds
+// at most C0_CMAX channels (grid.z walks the channel groups of wider layers): the backward kernels need up to ~80
+// registers per thread, so a 1024-thread block would not fit the 64 K register file and would not launch.
 // Checked on the device against oracle/speecht5_oracle_asr.py (tests/test_frontend_gpu.py) and, as an algorithm, through
 // its CPU restatement (tests/test_kernel_algorithms_cpu.py).
 #include "kernels.cuh"
@@ -17,13 +19,14 @@ namespace st5 {
 
 constexpr int C0_TCH = 128;   // output frames per block
 constexpr int C0_KMAX = 16;   // taps held in registers
+constexpr int C0_CMAX = 512;  // channels per block (launch bounds of the one-thread-per-channel kernels: <= 128 regs)
 
 __device__ __forceinline__ float c0_act(float z, int act) { return act == 4 ? gelu_tanh_fwd(z) : gelu_fwd(z); }
 
 // stages wave[b][t0*S .. t0*S + (nt-1)*S + K) and this thread's taps; returns the number of frames of the block
 __device__ __forceinline__ int c0_stage(const float* __restrict__ wave, const float* __restrict__ w, float* seg,
                                         float (&wr)[C0_KMAX], int64_t n, int T0, int C, int K, int S, int& t0) {
-  const int b = blockIdx.y, c = threadIdx.x;
+  const int b = blockIdx.y, c = blockIdx.z * blockDim.x + threadIdx.x;
   t0 = blockIdx.x * C0_TCH;
   const int nt = min(C0_TCH, T0 - t0);
   const int len = (nt - 1) * S + K;
@@ -43,13 +46,14 @@ __device__ __forceinline__ float c0_conv(const float* seg, const float (&wr)[C0_
 }
 
 // part[((b * chunks + chunk) * 2 + {0: sum, 1: centred sum of squares}) * C + c]
-__global__ void conv0_stats_kernel(const float* __restrict__ wave, const float* __restrict__ w, float* __restrict__ part,
-                                   int64_t n, int T0, int C, int K, int S) {
+__global__ void __launch_bounds__(C0_CMAX)
+    conv0_stats_kernel(const float* __restrict__ wave, const float* __restrict__ w, float* __restrict__ part, int64_t n,
+                       int T0, int C, int K, int S) {
   extern __shared__ float seg[];
   float wr[C0_KMAX];
   int t0;
   const int nt = c0_stage(wave, w, seg, wr, n, T0, C, K, S, t0);
-  const int c = threadIdx.x;
+  const int c = blockIdx.z * blockDim.x + threadIdx.x;
   if (c >= C) return;
   // one pass: sums of (v - pilot) and (v - pilot)^2 with the chunk's first value as the pilot, so the centred sum of
   // squares M2 = Q - S^2 / n is formed from numbers of the size of the deviations, not of the mean (the convolution
@@ -108,15 +112,15 @@ __global__ void __launch_bounds__(64 * C0_FG)
 }
 
 template <typename T>
-__global__ void conv0_apply_kernel(const float* __restrict__ wave, const float* __restrict__ w,
-                                   const float* __restrict__ gamma, const float* __restrict__ beta,
-                                   const float* __restrict__ mean, const float* __restrict__ rstd, T* __restrict__ y,
-                                   int64_t n, int T0, int C, int K, int S, int act) {
+__global__ void __launch_bounds__(C0_CMAX)
+    conv0_apply_kernel(const float* __restrict__ wave, const float* __restrict__ w, const float* __restrict__ gamma,
+                       const float* __restrict__ beta, const float* __restrict__ mean, const float* __restrict__ rstd,
+                       T* __restrict__ y, int64_t n, int T0, int C, int K, int S, int act) {
   extern __shared__ float seg[];
   float wr[C0_KMAX];
   int t0;
   const int nt = c0_stage(wave, w, seg, wr, n, T0, C, K, S, t0);
-  const int b = blockIdx.y, c = threadIdx.x;
+  const int b = blockIdx.y, c = blockIdx.z * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const float mu = mean[b * C + c];
   const float sc = rstd[b * C + c] * gamma[c];
@@ -130,16 +134,16 @@ __global__ void conv0_apply_kernel(const float* __restrict__ wave, const float* 
 
 // backward pass 1: part[.. * 2 + {0: sum g, 1: sum g * xhat}], g = dy * act'(z)
 template <typename T>
-__global__ void conv0_bwd_sums_kernel(const T* __restrict__ dy, const float* __restrict__ wave,
-                                      const float* __restrict__ w, const float* __restrict__ gamma,
-                                      const float* __restrict__ beta, const float* __restrict__ mean,
-                                      const float* __restrict__ rstd, float* __restrict__ part, int64_t n, int T0, int C,
-                                      int K, int S, int act) {
+__global__ void __launch_bounds__(C0_CMAX)
+    conv0_bwd_sums_kernel(const T* __restrict__ dy, const float* __restrict__ wave, const float* __restrict__ w,
+                          const float* __restrict__ gamma, const float* __restrict__ beta,
+                          const float* __restrict__ mean, const float* __restrict__ rstd, float* __restrict__ part,
+                          int64_t n, int T0, int C, int K, int S, int act) {
   extern __shared__ float seg[];
   float wr[C0_KMAX];
   int t0;
   const int nt = c0_stage(wave, w, seg, wr, n, T0, C, K, S, t0);
-  const int b = blockIdx.y, c = threadIdx.x;
+  const int b = blockIdx.y, c = blockIdx.z * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const float mu = mean[b * C + c], rs = rstd[b * C + c], ga = gamma[c], be = beta[c];
   const T* src = dy + ((int64_t)b * T0 + t0) * C + c;
@@ -189,16 +193,16 @@ __global__ void __launch_bounds__(64 * C0_FG)
 
 // backward pass 2: dv = rstd * gamma * (g - S1/T - xhat * S2/T); per-block partial dW[c][k] = sum_t dv[t] * wave[t*S + k]
 template <typename T>
-__global__ void conv0_bwd_w_kernel(const T* __restrict__ dy, const float* __restrict__ wave, const float* __restrict__ w,
-                                   const float* __restrict__ gamma, const float* __restrict__ beta,
-                                   const float* __restrict__ mean, const float* __restrict__ rstd,
-                                   const float* __restrict__ sums, float* __restrict__ part, int64_t n, int T0, int C,
-                                   int K, int S, int act) {
+__global__ void __launch_bounds__(C0_CMAX)
+    conv0_bwd_w_kernel(const T* __restrict__ dy, const float* __restrict__ wave, const float* __restrict__ w,
+                       const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+                       const float* __restrict__ rstd, const float* __restrict__ sums, float* __restrict__ part,
+                       int64_t n, int T0, int C, int K, int S, int act) {
   extern __shared__ float seg[];
   float wr[C0_KMAX];
   int t0;
   const int nt = c0_stage(wave, w, seg, wr, n, T0, C, K, S, t0);
-  const int b = blockIdx.y, c = threadIdx.x;
+  const int b = blockIdx.y, c = blockIdx.z * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const float mu = mean[b * C + c], rs = rstd[b * C + c], ga = gamma[c], be = beta[c];
   const float inv_t = 1.f / (float)T0;
@@ -222,8 +226,8 @@ __global__ void conv0_bwd_w_kernel(const T* __restrict__ dy, const float* __rest
 }
 
 // dw[i] += sum over the per-block partial rows (row range split over blockIdx.y, one atomic per thread)
-__global__ void conv0_reduce_w_kernel(const float* __restrict__ part, float* __restrict__ dw, int rows, int cols,
-                                      int64_t ld) {
+__global__ void __launch_bounds__(128)
+    conv0_reduce_w_kernel(const float* __restrict__ part, float* __restrict__ dw, int rows, int cols, int64_t ld) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= cols) return;
   const int per = (rows + gridDim.y - 1) / gridDim.y;
@@ -427,7 +431,12 @@ __global__ void __launch_bounds__(32 * C0L_WARPS)
 }
 
 static inline int c0_frames(int64_t n, int K, int S) { return n < K ? 0 : (int)((n - K) / S + 1); }
-static inline int c0_threads(int C) { return (C + 31) / 32 * 32; }
+// grid (chunks, B, channel groups), block: the channels of one group rounded up to whole warps
+static inline dim3 c0_grid(int chunks, int B, int C) { return dim3(chunks, B, (C + C0_CMAX - 1) / C0_CMAX); }
+static inline dim3 c0_block(int C) {
+  const int groups = (C + C0_CMAX - 1) / C0_CMAX;
+  return dim3(((C + groups - 1) / groups + 31) / 32 * 32);
+}
 
 int64_t conv0_ws_floats(int32_t B, int64_t n, int32_t C, int32_t K, int32_t S) {
   const int T0 = c0_frames(n, K, S);
@@ -449,7 +458,7 @@ int conv0_fwd_launch(const float* wave, const float* w, const float* gamma, cons
   if (rc) return rc;
   const int T0 = c0_frames(n, K, S);
   const int chunks = (T0 + C0_TCH - 1) / C0_TCH;
-  const dim3 grid(chunks, B), block(c0_threads(C));
+  const dim3 grid = c0_grid(chunks, B, C), block = c0_block(C);
   const size_t smem = ((size_t)(C0_TCH - 1) * S + K) * sizeof(float);
   if (smem > 48 * 1024) return -5;
   conv0_stats_kernel<<<grid, block, smem, st>>>(wave, w, ws, n, T0, C, K, S);
@@ -470,7 +479,7 @@ int conv0_bwd_launch(const void* dy, const float* wave, const float* w, const fl
   if (rc) return rc;
   const int T0 = c0_frames(n, K, S);
   const int chunks = (T0 + C0_TCH - 1) / C0_TCH;
-  const dim3 grid(chunks, B), block(c0_threads(C));
+  const dim3 grid = c0_grid(chunks, B, C), block = c0_block(C);
   const size_t smem = ((size_t)(C0_TCH - 1) * S + K) * sizeof(float);
   if (smem > 48 * 1024) return -5;
   float* sums = ws + (int64_t)B * chunks * C * (K > 2 ? K : 2);
@@ -478,12 +487,14 @@ int conv0_bwd_launch(const void* dy, const float* wave, const float* w, const fl
     const __nv_bfloat16* g = reinterpret_cast<const __nv_bfloat16*>(dy);
     conv0_bwd_sums_kernel<__nv_bfloat16><<<grid, block, smem, st>>>(g, wave, w, gamma, beta, mean, rstd, ws, n, T0, C, K,
                                                                     S, act);
+    if (const cudaError_t e = cudaGetLastError()) return (int)e;  // nothing accumulated yet
     conv0_bwd_finalize_kernel<<<dim3(B, (C + 63) / 64), dim3(64, C0_FG), 0, st>>>(ws, sums, dgamma, dbeta, C, chunks);
     conv0_bwd_w_kernel<__nv_bfloat16><<<grid, block, smem, st>>>(g, wave, w, gamma, beta, mean, rstd, sums, ws, n, T0, C,
                                                                  K, S, act);
   } else {
     const float* g = reinterpret_cast<const float*>(dy);
     conv0_bwd_sums_kernel<float><<<grid, block, smem, st>>>(g, wave, w, gamma, beta, mean, rstd, ws, n, T0, C, K, S, act);
+    if (const cudaError_t e = cudaGetLastError()) return (int)e;  // nothing accumulated yet
     conv0_bwd_finalize_kernel<<<dim3(B, (C + 63) / 64), dim3(64, C0_FG), 0, st>>>(ws, sums, dgamma, dbeta, C, chunks);
     conv0_bwd_w_kernel<float><<<grid, block, smem, st>>>(g, wave, w, gamma, beta, mean, rstd, sums, ws, n, T0, C, K, S,
                                                          act);

@@ -136,6 +136,18 @@ def backward(f, dO, dP_ext=None):
     return g
 
 
+def score_error(f, Cs):
+    """Relative error of each exp(s - rowmax) from the fp32 score and exponent argument (see `bounds`)."""
+    q, k, sc = f["q"], f["k"], f["scale"]
+    aq, ak = q.abs(), k.abs()
+    smag = sc * (aq @ ak.transpose(-1, -2))
+    if f["pe"] is not None:
+        smag = smag + sc * _qpe(aq, f["pe"].abs(), k.shape[2], f["maxpos"], f["rows"])
+    s_abs = torch.where(f["ok"], f["s"].abs(), torch.zeros_like(smag))
+    smag = torch.where(f["ok"], smag, torch.zeros_like(smag))
+    return Cs * 2.0 ** -24 * (smag + s_abs + (smag + s_abs).amax(-1, keepdim=True) + 4.0)
+
+
 def bounds(f, g=None, *, u, C, Cs=64.0):
     """Elementwise bounds, same shapes as the quantities. `u`: storage unit roundoff; `C`: constant set on the H100.
 
@@ -144,13 +156,7 @@ def bounds(f, g=None, *, u, C, Cs=64.0):
     EP = P * Cs 2^-24 (Smag_ij + |s_ij| + max_j (Smag + |s|) + 4)."""
     q, k, v, sc = f["q"], f["k"], f["v"], f["scale"]
     aq, ak, av = q.abs(), k.abs(), v.abs()
-    Tk = k.shape[2]
-    smag = sc * (aq @ ak.transpose(-1, -2))
-    if f["pe"] is not None:
-        smag = smag + sc * _qpe(aq, f["pe"].abs(), Tk, f["maxpos"], f["rows"])
-    s_abs = torch.where(f["ok"], f["s"].abs(), torch.zeros_like(smag))
-    smag = torch.where(f["ok"], smag, torch.zeros_like(smag))
-    es = Cs * 2.0 ** -24 * (smag + s_abs + (smag + s_abs).amax(-1, keepdim=True) + 4.0)
+    es = score_error(f, Cs)
     P, Pd = f["P"], f["Pd"]
     EP = P * es
     EPd = EP * f["keep"] * f["dscale"]
@@ -174,6 +180,38 @@ def bounds(f, g=None, *, u, C, Cs=64.0):
         b["dQP"] = BQP + u * g["dQP"].abs() + TINY
         b["dQ"] = b["dQ_k"] + sc * (BQP @ f["pe"].abs()) + u * g["dQ"].abs()
         b["dPE"] = sc * torch.einsum("bhir,bhic->rc", BQP, aq) + u * g["dPE"].abs() + TINY
+    return b
+
+
+# ============================================================================================ decode (Tq = 1)
+DCH = 64  # keys per split of st5_attn_decode_fwd
+
+
+def decode_forward(q, k, v, *, scale, key_pad=None):
+    """st5_attn_decode_fwd: q [B, H, 64], k / v [B, H, Tk, 64] -> out [B, H, 64] and P [B, H, Tk] = softmax over the
+    unmasked keys of each (b, h). A (b, h) with every key masked gives zeros (out and P), as the header states."""
+    f = forward(q[:, :, None], k, v, scale=scale, key_pad=key_pad)
+    dead = ~f["ok"].any(-1)                                    # [B, H, 1]
+    f["P"] = f["P"].masked_fill(dead[..., None], 0.0)
+    f["Pd"] = f["P"]
+    f["out"] = f["out"].masked_fill(dead[..., None], 0.0)
+    f["dead"] = dead[..., 0]
+    return f
+
+
+def decode_bounds(f, *, u):
+    """Elementwise bounds of out (storage unit u) and the fp32 probabilities, from `score_error` (64-term dot
+    products: <= 8 sequential products per lane + 4 shuffle levels; the exponent; the merge factor exp(m_s - M)) and the
+    fp32 sums: within a split, the denominator is a 5-level shuffle tree plus 4 warp partials and each output channel
+    <= 8 sequential keys per lane, <= 2 shuffle levels and 4 warp partials; the splits are then merged in index order,
+    one more level each (depth ns)."""
+    P, av = f["P"], f["v"].abs()
+    ns = -(-f["k"].shape[2] // DCH)
+    es = score_error(f, 64.0)
+    el = es.amax(-1, keepdim=True) + (ns + 16) * 2.0 ** -24          # relative error of the denominator L
+    EP = P * (es + el + 2 * 2.0 ** -24)
+    b = {"P": (EP + TINY)[:, :, 0]}
+    b["out"] = ((ns + 24) * 2.0 ** -24 * (P @ av) + EP @ av + u * f["out"].abs() + TINY)[:, :, 0]
     return b
 
 
