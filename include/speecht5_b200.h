@@ -213,6 +213,57 @@ typedef struct st5_attn_decode_args {
 int64_t st5_attn_decode_ws_floats(int32_t B, int32_t H, int32_t Tk, int32_t with_probs);
 int st5_attn_decode_fwd(const st5_attn_decode_args* args, void* stream);
 
+/* One-query-row attention for beam search (sequence_generator.py:327-361, reorder_incremental_state): the same kernel and
+ * contract as st5_attn_decode_fwd, except that key / value j of query row b is read from batch row
+ *   kv_rows[b * kv_rows_ld + j]   when kv_rows != NULL (kv_div must then be 1, kv_rows_ld >= Tk), else
+ *   b / kv_div                     (kv_div >= 1).
+ * The first form is the decoder self-attention over a lineage table (each cache cell is written once; a beam reorder
+ * rewrites the table, not the cache), the second the cross-attention of K beams over one copy of their sentence's encoder
+ * keys / values (kv_div = K). base.B is the number of query rows; key_pad is indexed by query row. Returns -2 for a bad
+ * kv_div / kv_rows_ld, otherwise the codes of st5_attn_decode_fwd. */
+typedef struct st5_attn_lineage_args {
+  st5_attn_decode_args base;
+  const int32_t* kv_rows;      /* [B][kv_rows_ld] or NULL */
+  int64_t kv_rows_ld;
+  int32_t kv_div;
+} st5_attn_lineage_args;
+int st5_attn_lineage_fwd(const st5_attn_lineage_args* args, void* stream);
+
+/* Beam search candidate selection (sequence_generator.py:430-454 with fairseq/search.py:117-144, BeamSearch.step) for B
+ * sentences of K beams (1 <= K <= 16, rows r = s * K + k), vocabulary V (1 < V <= 32768). Per row, fp32:
+ *   lp = x / T - logsumexp(x / T)   (x = logits[r * ld + v], ST5_F32 or ST5_BF16; inv_temp = 1 / T)
+ *   eos -> -inf while *t < *min_len; NaN -> -inf; lp += mask[v]; every v != eos -> -inf once *t >= *max_len;
+ *   lp += cum[r] for *t > 0 (at *t == 0 only beam 0 of each sentence takes part).
+ * Per sentence the best n = min(2K, F - 1) of the F = (t == 0 ? V : K * V) flat candidates (beam * V + v), in
+ * descending score, ties to the lower flat index: cand_score / cand_token / cand_beam[s * 2K + i], i < n; entries
+ * i >= n are not written. t, min_len, max_len are device scalars (a captured graph replays any step).
+ * ws: st5_beam_topk_ws_floats(B, K) floats of scratch. Returns -2 for K, V or B out of range, -3 for a NULL pointer,
+ * -6 unless ld >= V; nothing is launched then. */
+int64_t st5_beam_topk_ws_floats(int32_t B, int32_t K);
+int st5_beam_topk(const void* logits, int64_t ld, int dtype, int32_t B, int32_t K, int32_t V, const float* cum,
+                  const float* mask, float inv_temp, int32_t eos, const int64_t* t, const int64_t* min_len,
+                  const int64_t* max_len, float* cand_score, int32_t* cand_token, int32_t* cand_beam, float* ws,
+                  void* stream);
+
+/* Beam search bookkeeping for step *t (sequence_generator.py:487-636 with finalize_hypos / is_finished :690-816), one
+ * CTA per sentence; a sentence with finished[s] != 0 is skipped. State of slot r (= s * K + k), capacity T positions:
+ *   lin[r][j]  the slot whose cells hold position j of the hypothesis now in slot r (lin[r][t] == r on entry);
+ *   tok[r][j], score[r][j]  the token at position j (j >= 1; position 0 is the initial eos) and the cumulative score
+ *   after it, stored in the cell (lin, j) of the slot that chose it.
+ * ignore[s][K]: cands_to_ignore (by candidate position). Finalized hypotheses: fin_n[s] (count), fin_tok[s][K][T],
+ * fin_pos[s][K][T] (positional scores = differences of the cumulative fp32 scores), fin_len[s][K], fin_score[s][K]
+ * (eos score / (t + 1) ** len_penalty when normalize). For each eos candidate among the first K (score > -inf, not
+ * ignored) the hypothesis is appended while fin_n < K; the sentence is finished at fin_n == K or t == max_len.
+ * Otherwise the first K non-eos candidates (then eos ones, which become ignored) continue: parent[r], cur_tok[r],
+ * cur_score[r], lin[r][0..t] = lin[parent][0..t], lin[r][t+1] = r, tok / score[r][t+1]. stop[*t] = 1 when every
+ * sentence is finished. t + 2 <= T is required (the caller sizes T). Returns -2 for K / T out of range, -3 for a NULL
+ * pointer. */
+int st5_beam_update(int32_t B, int32_t K, int32_t V, int32_t T, int32_t eos, const int64_t* t, const int64_t* max_len,
+                    int32_t normalize, float len_penalty, const float* cand_score, const int32_t* cand_token,
+                    const int32_t* cand_beam, int32_t* lin, int32_t* tok, float* score, int32_t* ignore,
+                    int32_t* finished, int32_t* parent, int64_t* cur_tok, float* cur_score, int32_t* fin_n,
+                    int32_t* fin_tok, float* fin_pos, int32_t* fin_len, float* fin_score, int32_t* stop, void* stream);
+
 /* Fused wgmma attention forward (bf16, Tk <= 320): QK^T -> masks -> softmax -> dropout -> PV in ONE launch, no score
  * or probability round trip through HBM. Uses the q/k/v/out/probs/key_pad/scale/dropout fields of st5_attn_args exactly
  * like st5_attn_fwd; additionally writes lse[b][h][i] = log sum_j exp(s_ij) over the keys row i sees (natural log, the

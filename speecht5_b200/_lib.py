@@ -58,6 +58,10 @@ class AttnDecodeArgs(C.Structure):
     ]
 
 
+class AttnLineageArgs(C.Structure):
+    _fields_ = [("base", AttnDecodeArgs), ("kv_rows", C.c_void_p), ("kv_rows_ld", C.c_int64), ("kv_div", C.c_int32)]
+
+
 _vp, _i64, _i32, _f, _u64 = C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_uint64
 _PROTOS = {
     "st5_version": (C.c_int, []),
@@ -80,6 +84,11 @@ _PROTOS = {
     "st5_attn_bwd": (C.c_int, [C.POINTER(AttnArgs), _vp]),
     "st5_attn_decode_ws_floats": (C.c_int64, [_i32, _i32, _i32, _i32]),
     "st5_attn_decode_fwd": (C.c_int, [C.POINTER(AttnDecodeArgs), _vp]),
+    "st5_attn_lineage_fwd": (C.c_int, [C.POINTER(AttnLineageArgs), _vp]),
+    "st5_beam_topk_ws_floats": (C.c_int64, [_i32, _i32]),
+    "st5_beam_topk": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _f, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                _vp]),
+    "st5_beam_update": (C.c_int, [_i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _f] + [_vp] * 18),
     "st5_attn_fused_fwd": (C.c_int, [C.POINTER(AttnArgs), _vp, _vp, _vp, _vp, _vp]),
     "st5_attn_flash_fwd": (C.c_int, [C.POINTER(AttnArgs), _vp, _vp, _vp, _vp, _vp]),
     "st5_attn_fused_bwd": (C.c_int, [C.POINTER(AttnArgs), _vp, _vp, _vp, _vp, _vp, _i32, _vp]),

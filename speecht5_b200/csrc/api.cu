@@ -136,6 +136,29 @@ int64_t st5_attn_decode_ws_floats(int32_t B, int32_t H, int32_t Tk, int32_t with
 int st5_attn_decode_fwd(const st5_attn_decode_args* a, void* stream) {
   return set_error(attn_decode_launch(*a, (cudaStream_t)stream), "st5_attn_decode_fwd");
 }
+int st5_attn_lineage_fwd(const st5_attn_lineage_args* a, void* stream) {
+  return set_error(attn_lineage_launch(*a, (cudaStream_t)stream), "st5_attn_lineage_fwd");
+}
+
+int64_t st5_beam_topk_ws_floats(int32_t B, int32_t K) { return beam_topk_ws_floats(B, K); }
+int st5_beam_topk(const void* logits, int64_t ld, int dtype, int32_t B, int32_t K, int32_t V, const float* cum,
+                  const float* mask, float inv_temp, int32_t eos, const int64_t* t, const int64_t* min_len,
+                  const int64_t* max_len, float* cand_score, int32_t* cand_token, int32_t* cand_beam, float* ws,
+                  void* stream) {
+  return set_error(beam_topk_launch(logits, ld, dtype, B, K, V, cum, mask, inv_temp, eos, t, min_len, max_len,
+                                    cand_score, cand_token, cand_beam, ws, (cudaStream_t)stream),
+                   "st5_beam_topk");
+}
+int st5_beam_update(int32_t B, int32_t K, int32_t V, int32_t T, int32_t eos, const int64_t* t, const int64_t* max_len,
+                    int32_t normalize, float len_penalty, const float* cand_score, const int32_t* cand_token,
+                    const int32_t* cand_beam, int32_t* lin, int32_t* tok, float* score, int32_t* ignore,
+                    int32_t* finished, int32_t* parent, int64_t* cur_tok, float* cur_score, int32_t* fin_n,
+                    int32_t* fin_tok, float* fin_pos, int32_t* fin_len, float* fin_score, int32_t* stop, void* stream) {
+  return set_error(beam_update_launch(B, K, V, T, eos, t, max_len, normalize, len_penalty, cand_score, cand_token,
+                                      cand_beam, lin, tok, score, ignore, finished, parent, cur_tok, cur_score, fin_n,
+                                      fin_tok, fin_pos, fin_len, fin_score, stop, (cudaStream_t)stream),
+                   "st5_beam_update");
+}
 
 int st5_bn_fwd(const void* x, int64_t x_ld, const float* gamma, const float* beta, float* running_mean,
                float* running_var, float* save_mean, float* save_rstd, void* y, int64_t y_ld, void* y_pre, int dtype,

@@ -55,10 +55,18 @@ __device__ __forceinline__ float cta_reduce(float v, float* red, bool is_max) {
   return r;
 }
 
+// Where key / value j of query row b lives. Plain (st5_attn_decode_fwd): batch row b. Lineage (st5_attn_lineage_fwd):
+// batch row rows[b * rows_ld + j] when a table is given, else b / div.
+struct KvMap {
+  const int32_t* rows;
+  int64_t rows_ld;
+  int div;
+};
+
 // direct != 0: the buffer holds at most DCH keys, so there is one split and this CTA writes the final output (and
 // probabilities) itself -- bit-identical to what the combine kernel makes of a single split.
-template <typename T>
-__global__ void __launch_bounds__(DT) attn_decode_split(const st5_attn_decode_args a, int n_splits, int direct) {
+template <typename T, bool MAP>
+__device__ __forceinline__ void decode_split(const st5_attn_decode_args& a, const KvMap& map, int n_splits, int direct) {
   constexpr int VE = Vec16<T>::N;   // elements per 16-byte load
   constexpr int LPK = DH / VE;      // lanes per key row
   constexpr int KPI = DT / LPK;     // keys per CTA iteration
@@ -76,7 +84,9 @@ __global__ void __launch_bounds__(DT) attn_decode_split(const st5_attn_decode_ar
 #pragma unroll
   for (int e = 0; e < VE; ++e) qr[e] = q[sub * VE + e];
   const uint8_t* kp = a.key_pad != nullptr ? a.key_pad + (int64_t)b * a.Tk : nullptr;
-  const T* kb = (const T*)a.k + (int64_t)b * a.k_bs + h * DH + sub * VE;
+  const int32_t* rt = MAP && map.rows != nullptr ? map.rows + (int64_t)b * map.rows_ld : nullptr;
+  const int64_t kvb = MAP ? (int64_t)(b / map.div) : (int64_t)b;
+  const T* kb = (const T*)a.k + h * DH + sub * VE;
 #pragma unroll
   for (int it = 0; it < DCH / KPI; ++it) {
     const int j = j0 + it * KPI + slot;
@@ -84,7 +94,7 @@ __global__ void __launch_bounds__(DT) attn_decode_split(const st5_attn_decode_ar
     float d = 0.f;
     if (valid) {
       float kr[VE];
-      Vec16<T>::load(kb + (int64_t)j * a.k_ld, kr);
+      Vec16<T>::load(kb + (MAP && rt != nullptr ? (int64_t)rt[j] : kvb) * a.k_bs + (int64_t)j * a.k_ld, kr);
 #pragma unroll
       for (int e = 0; e < VE; ++e) d += qr[e] * kr[e];
     }
@@ -102,7 +112,7 @@ __global__ void __launch_bounds__(DT) attn_decode_split(const st5_attn_decode_ar
   if (!direct && a.probs != nullptr && tid < DCH && j0 + tid < a.Tk) a.ws[(int64_t)n_splits * DPART * a.B * a.H + bh * a.Tk + j0 + tid] = sraw;
   __syncthreads();
   // out_c = sum_j e_j v_jc: lane `sub` owns channels sub*VE .. +VE, slots stride over the split's keys
-  const T* vb = (const T*)a.v + (int64_t)b * a.v_bs + h * DH + sub * VE;
+  const T* vb = (const T*)a.v + h * DH + sub * VE;
   float acc[VE];
 #pragma unroll
   for (int e = 0; e < VE; ++e) acc[e] = 0.f;
@@ -112,7 +122,8 @@ __global__ void __launch_bounds__(DT) attn_decode_split(const st5_attn_decode_ar
     const float p = sc[jj];
     if (j0 + jj < j1 && p != 0.f) {
       float vr[VE];
-      Vec16<T>::load(vb + (int64_t)(j0 + jj) * a.v_ld, vr);
+      const int j = j0 + jj;
+      Vec16<T>::load(vb + (MAP && rt != nullptr ? (int64_t)rt[j] : kvb) * a.v_bs + (int64_t)j * a.v_ld, vr);
 #pragma unroll
       for (int e = 0; e < VE; ++e) acc[e] += p * vr[e];
     }
@@ -146,6 +157,16 @@ __global__ void __launch_bounds__(DT) attn_decode_split(const st5_attn_decode_ar
       for (int j = tid; j < a.Tk; j += DT) pr[j] = sc[j] * inv;
     }
   }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(DT) attn_decode_split(const st5_attn_decode_args a, int n_splits, int direct) {
+  decode_split<T, false>(a, KvMap{nullptr, 0, 1}, n_splits, direct);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(DT) attn_lineage_split(const st5_attn_lineage_args a, int n_splits, int direct) {
+  decode_split<T, true>(a.base, KvMap{a.kv_rows, a.kv_rows_ld, a.kv_div}, n_splits, direct);
 }
 
 __global__ void __launch_bounds__(DT) attn_decode_combine(const st5_attn_decode_args a, int n_splits, int dtype) {
@@ -184,20 +205,41 @@ int64_t attn_decode_ws_floats(int B, int H, int Tk, int with_probs) {
   return (int64_t)B * H * (ns * DPART + (with_probs ? Tk : 0));
 }
 
-int attn_decode_launch(const st5_attn_decode_args& a, cudaStream_t st) {
+static int decode_check(const st5_attn_decode_args& a) {
   if (a.B <= 0 || a.H <= 0 || a.Tk <= 0) return -2;
   const int esz = a.dtype == ST5_F32 ? 4 : 2;
   if (((a.k_ld * esz) & 15) || ((a.v_ld * esz) & 15) || ((a.k_bs * esz) & 15) || ((a.v_bs * esz) & 15)) return -6;
   if ((reinterpret_cast<uintptr_t>(a.k) & 15) || (reinterpret_cast<uintptr_t>(a.v) & 15)) return -6;
+  if (a.Tk > DCH && a.ws == nullptr) return -5;
+  return 0;
+}
+
+int attn_decode_launch(const st5_attn_decode_args& a, cudaStream_t st) {
+  const int rc = decode_check(a);
+  if (rc != 0) return rc;
   const int ns = (a.Tk + DCH - 1) / DCH;
   const int direct = ns == 1;
-  if (!direct && a.ws == nullptr) return -5;
   const dim3 grid(ns, a.H, a.B);
   if (a.dtype == ST5_F32) attn_decode_split<float><<<grid, DT, 0, st>>>(a, ns, direct);
   else attn_decode_split<__nv_bfloat16><<<grid, DT, 0, st>>>(a, ns, direct);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || direct) return (int)e;
   attn_decode_combine<<<dim3(a.H, a.B), DT, 0, st>>>(a, ns, a.dtype);
+  return (int)cudaGetLastError();
+}
+
+int attn_lineage_launch(const st5_attn_lineage_args& a, cudaStream_t st) {
+  const int rc = decode_check(a.base);
+  if (rc != 0) return rc;
+  if (a.kv_div < 1 || (a.kv_rows != nullptr && (a.kv_div != 1 || a.kv_rows_ld < a.base.Tk))) return -2;
+  const int ns = (a.base.Tk + DCH - 1) / DCH;
+  const int direct = ns == 1;
+  const dim3 grid(ns, a.base.H, a.base.B);
+  if (a.base.dtype == ST5_F32) attn_lineage_split<float><<<grid, DT, 0, st>>>(a, ns, direct);
+  else attn_lineage_split<__nv_bfloat16><<<grid, DT, 0, st>>>(a, ns, direct);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess || direct) return (int)e;
+  attn_decode_combine<<<dim3(a.base.H, a.base.B), DT, 0, st>>>(a.base, ns, a.base.dtype);
   return (int)cudaGetLastError();
 }
 

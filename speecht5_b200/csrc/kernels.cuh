@@ -147,6 +147,17 @@ int attn_fwd_launch(const st5_attn_args& a, cudaStream_t s);
 int attn_bwd_launch(const st5_attn_args& a, cudaStream_t s);
 int64_t attn_decode_ws_floats(int B, int H, int Tk, int with_probs);
 int attn_decode_launch(const st5_attn_decode_args& a, cudaStream_t s);
+int attn_lineage_launch(const st5_attn_lineage_args& a, cudaStream_t s);
+int64_t beam_topk_ws_floats(int B, int K);
+int beam_topk_launch(const void* logits, int64_t ld, int dtype, int B, int K, int V, const float* cum,
+                     const float* mask, float inv_temp, int eos, const int64_t* t, const int64_t* min_len,
+                     const int64_t* max_len, float* cand_score, int32_t* cand_token, int32_t* cand_beam, float* ws,
+                     cudaStream_t s);
+int beam_update_launch(int B, int K, int V, int T, int eos, const int64_t* t, const int64_t* max_len, int normalize,
+                       float len_penalty, const float* cand_score, const int32_t* cand_token, const int32_t* cand_beam,
+                       int32_t* lin, int32_t* tok, float* score, int32_t* ignore, int32_t* finished, int32_t* parent,
+                       int64_t* cur_tok, float* cur_score, int32_t* fin_n, int32_t* fin_tok, float* fin_pos,
+                       int32_t* fin_len, float* fin_score, int32_t* stop, cudaStream_t s);
 int bn_fwd_launch(const void* x, int64_t x_ld, const float* gamma, const float* beta, float* running_mean,
                   float* running_var, float* save_mean, float* save_rstd, void* y, int64_t y_ld, void* y_pre, int dtype,
                   int64_t rows, int64_t C, int training, float momentum, float eps, int act, float drop_p,

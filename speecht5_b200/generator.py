@@ -3,8 +3,9 @@
 speecht5/sequence_generator.py:207-655 with ctc_weight 0 and no LM is `T5TransformerModel.generate_text_greedy`; this
 class gives it the SequenceGenerator call / return shape (:191-205, :596-655: a list over sentences of a list over beams
 of {"tokens", "score", "attention", "alignment", "positional_scores"}, score = sum of the token log-probabilities
-divided by length ** len_penalty when normalize_scores is on). Beam search > 1, LM fusion and CTC rescoring are out of
-scope (SURVEY section 2) and raise."""
+divided by length ** len_penalty when normalize_scores is on). Beam search > 1 is BeamSearchGenerator
+(`task.build_generator(models, args, seq_gen_cls=BeamSearchGenerator)`); LM fusion and CTC rescoring are out of scope
+(SURVEY section 2) and raise."""
 import torch
 
 
@@ -43,3 +44,35 @@ class GreedyGenerator:
             out.append([{"tokens": tok, "score": total, "attention": None, "alignment": torch.empty(0),
                          "positional_scores": pos}])
         return out
+
+
+class BeamSearchGenerator:
+    """The SequenceGenerator of sequence_generator.py:207-654 for beam_size K >= 2 (ctc_weight 0, no LM, no prefix tokens
+    or constraints) on T5TransformerModel.generate_text_beam; same keywords as GreedyGenerator. beam_size 1 is
+    GreedyGenerator itself. use_cache: True (eager step body) or "graph" (one captured CUDA graph per step)."""
+
+    def __init__(self, models, tgt_dict, beam_size=5, max_len_a=0, max_len_b=200, min_len=1, normalize_scores=True,
+                 len_penalty=1.0, unk_penalty=0.0, temperature=1.0, ctc_weight=0.0, lm_model=None, use_cache=True,
+                 blank=None, mask_idx=None, **unused):
+        kw = dict(max_len_a=max_len_a, max_len_b=max_len_b, min_len=min_len, normalize_scores=normalize_scores,
+                  len_penalty=len_penalty, unk_penalty=unk_penalty, temperature=temperature, ctc_weight=ctc_weight,
+                  lm_model=lm_model, use_cache=use_cache, blank=blank, mask_idx=mask_idx)
+        # (GreedyGenerator checks the options this class shares with it: CTC weight, LM)
+        self.greedy = GreedyGenerator(models, tgt_dict, beam_size=1, **kw)
+        self.beam_size = int(beam_size)
+        if self.beam_size != 1 and use_cache not in (True, "graph"):
+            raise ValueError(f"beam search runs with use_cache=True or 'graph', got {use_cache!r}")
+
+    @torch.no_grad()
+    def generate(self, models, sample, prefix_tokens=None, constraints=None, bos_token=None):
+        g = self.greedy
+        if self.beam_size == 1:
+            return g.generate(models, sample, prefix_tokens=prefix_tokens, constraints=constraints, bos_token=bos_token)
+        if prefix_tokens is not None or constraints is not None:
+            raise NotImplementedError("prefix tokens / constraints are not built for beam search")
+        ni = sample["net_input"]
+        return g.model.generate_text_beam(
+            ni["source"], ni.get("padding_mask"), beam_size=self.beam_size, max_len_a=g.max_len_a,
+            max_len_b=g.max_len_b, min_len=g.min_len, unk_penalty=g.unk_penalty, temperature=g.temperature, pad=g.pad,
+            eos=g.eos, unk=g.unk, blank=g.blank, mask_idx=g.mask_idx, use_cache=g.use_cache,
+            normalize_scores=g.normalize_scores, len_penalty=g.len_penalty)

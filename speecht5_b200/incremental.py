@@ -12,7 +12,7 @@ GEMM, the one-row attention on the split-KV decode kernel (st5_attn_decode_fwd),
 views."""
 import torch
 
-from . import ops
+from . import kernels, ops
 from .ops import RT
 
 
@@ -56,13 +56,18 @@ class DecoderCache:
 
 
 @torch.no_grad()
-def decoder_step(decoder, x_new, cache, need_head_weights=False, t_dev=None, span=None, self_pad=None):
+def decoder_step(decoder, x_new, cache, need_head_weights=False, t_dev=None, span=None, self_pad=None, self_rows=None,
+                 cross_div=1):
     """x_new [B, 1, C] = decoder-prenet output of the newest position. Returns (x [B, 1, C], [attn [B, H, 1, S]] per
     layer or None). Evaluation semantics (no dropout, no LayerDrop) -- generation only.
 
     Device-side step index (the form a captured graph replays): `t_dev` int64 [1] holds the position, the new key / value
     row is written with index_copy_, and self-attention runs over the first `span` cache rows with `self_pad` (uint8
-    [B, span], 1 = position > t) masking what has not been written yet -- no host scalar depends on the step."""
+    [B, span], 1 = position > t) masking what has not been written yet -- no host scalar depends on the step.
+
+    Beam search (BeamGraph, device-step form only): `self_rows` int32 [B, >= span] is the lineage table -- key j of row b
+    is read from cache row self_rows[b, j] -- and with cross_div = K row b attends over cross keys / values row b // K
+    (one copy per sentence). Neither returns attention probabilities."""
     assert not decoder.training
     x = _act_dtype(x_new).contiguous()
     t = cache.t
@@ -79,6 +84,10 @@ def decoder_step(decoder, x_new, cache, need_head_weights=False, t_dev=None, spa
             cache.self_kv[li][:, t] = qkv[:, 0, C:]
             a, _ = _attend(qkv, cache.self_kv[li][:, : t + 1], H=sa.num_heads, d=C, q_col=0, k_col=0, v_col=1,
                            scale=sa.scaling)
+        elif self_rows is not None:
+            cache.self_kv[li].index_copy_(1, t_dev, qkv[:, :, C:])
+            a, _ = ops.attention_decode(qkv, cache.self_kv[li][:, :span], H=sa.num_heads, d=C, q_col=0, k_col=0, v_col=1,
+                                        scale=sa.scaling, key_pad=self_pad, kv_rows=self_rows)
         else:
             cache.self_kv[li].index_copy_(1, t_dev, qkv[:, :, C:])
             a, _ = _attend(qkv, cache.self_kv[li][:, :span], H=sa.num_heads, d=C, q_col=0, k_col=0, v_col=1,
@@ -91,8 +100,12 @@ def decoder_step(decoder, x_new, cache, need_head_weights=False, t_dev=None, spa
         residual = x
         h = ops.residual_layer_norm(x, None, layer.encoder_attn_layer_norm) if layer.normalize_before else x
         q = ops.linear(h, ca.q_proj.weight, ca.q_proj.bias)
-        a, probs = _attend(q, cache.cross[li], H=ca.num_heads, d=C, q_col=0, k_col=0, v_col=1, scale=ca.scaling,
-                           key_pad=cache.enc_pad, return_probs=need_head_weights)
+        if cross_div != 1:
+            a, probs = ops.attention_decode(q, cache.cross[li], H=ca.num_heads, d=C, q_col=0, k_col=0, v_col=1,
+                                            scale=ca.scaling, key_pad=cache.enc_pad, kv_div=cross_div)
+        else:
+            a, probs = _attend(q, cache.cross[li], H=ca.num_heads, d=C, q_col=0, k_col=0, v_col=1, scale=ca.scaling,
+                               key_pad=cache.enc_pad, return_probs=need_head_weights)
         if need_head_weights:
             attns.append(probs.float())
         if layer.normalize_before:
@@ -478,3 +491,159 @@ def greedy_graph(model, B, S, max_len, device, capture=True):
             del store[k]
         gg = store[key] = GreedyGraph(model, B, S_b, M_b, device, capture=capture)
     return gg
+
+
+class BeamGraph:
+    """Beam search for text output (speecht5/sequence_generator.py:207-654 with ctc_weight 0, no LM, no prefix tokens;
+    candidate selection fairseq/search.py:117-144) over B sentences x K beams = B*K decoder rows, every step = ONE
+    CUDA-graph replay: embedding + position row of each row's newest token, the key/value-cached decoder, the vocabulary
+    projection, st5_beam_topk (log-softmax, the reference's masking, the best min(2K, F-1) candidates per sentence) and
+    st5_beam_update (finalize, is_finished, active selection, reorder) -- all on the device.
+
+    The batch stays B*K rows: a finished sentence is skipped by the bookkeeping and what its rows still compute is never
+    read (the reference drops it; every per-sentence quantity depends on that sentence only). A reorder never copies the
+    key/value cache: each (row, position) cell is written once, and the lineage table lin[row][position] -- the
+    self-attention's kv_rows -- says which row's cell holds each position of a hypothesis. Cross keys / values are
+    projected once per sentence into [B, S, 2C]; the K beams read them with kv_div = K. Utterance-independent like
+    GreedyGraph: encoder length and step budget are buckets. capture=False runs the same step body eagerly."""
+
+    CHUNK = 8
+
+    def __init__(self, model, B, K, S_bucket, maxlen_bucket, device, capture=True):
+        self.m, self.capture = model, capture
+        dec = model.decoder
+        dev = torch.device(device)
+        self.dev, self.B, self.K, self.S, self.maxlen = dev, int(B), int(K), int(S_bucket), int(maxlen_bucket)
+        B, K = self.B, self.K
+        BK = B * K
+        rows = self.maxlen + 1 + self.CHUNK
+        C = dec.layers[0].self_attn.embed_dim
+        self.cache = _StaticCache([torch.zeros((B, self.S, 2 * C), dtype=RT.dtype, device=dev) for _ in dec.layers],
+                                  [torch.zeros((BK, rows, 2 * C), dtype=RT.dtype, device=dev) for _ in dec.layers],
+                                  torch.zeros((BK, self.S), dtype=torch.uint8, device=dev), rows)
+        self.V = model.text_decoder_postnet.output_projection.weight.shape[0]
+        i32, f32 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.float32, device=dev)
+        self.state = dict(
+            t=torch.zeros(1, dtype=torch.int64, device=dev), max_len=torch.zeros(1, dtype=torch.int64, device=dev),
+            cand_score=torch.zeros((B, 2 * K), **f32), cand_token=torch.zeros((B, 2 * K), **i32),
+            cand_beam=torch.zeros((B, 2 * K), **i32), lin=torch.zeros((BK, rows), **i32),
+            tok=torch.zeros((BK, rows), **i32), score=torch.zeros((BK, rows), **f32), ignore=torch.zeros(BK, **i32),
+            finished=torch.zeros(B, **i32), parent=torch.zeros(BK, **i32),
+            cur_tok=torch.zeros(BK, dtype=torch.int64, device=dev), cur_score=torch.zeros(BK, **f32),
+            fin_n=torch.zeros(B, **i32), fin_tok=torch.zeros((B, K, rows), **i32),
+            fin_pos=torch.zeros((B, K, rows), **f32), fin_len=torch.zeros((B, K), **i32),
+            fin_score=torch.zeros((B, K), **f32), stop=torch.zeros(rows, **i32))
+        self.t, self.stop = self.state["t"], self.state["stop"]
+        self.min_len = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.mask = torch.zeros(self.V, dtype=torch.float32, device=dev)  # pad / blank / mask symbol never, unk penalty
+        self.pos = torch.arange(rows, device=dev)
+        self.pe = model.text_decoder_prenet._table(rows, dev)
+        self.consts = None  # (eos, 1 / temperature, normalize, len_penalty): host arguments the graphs bake
+        self.graphs = {}
+        self.stream = torch.cuda.Stream(device=dev) if capture else None
+        self.dtype = RT.dtype
+
+    @torch.no_grad()
+    def begin(self, encoder_out, max_len, min_len, unk_penalty, temperature, pad, eos, unk, blank, mask_idx,
+              normalize_scores, len_penalty):
+        import math
+        enc = encoder_out.get("_encoder_out_btc")
+        if enc is None:
+            enc = encoder_out["encoder_out"][0].transpose(0, 1).contiguous()
+        enc = _act_dtype(enc)
+        B, S = enc.shape[0], enc.shape[1]
+        assert B == self.B and S <= self.S and max_len <= self.maxlen and RT.dtype == self.dtype
+        pm = encoder_out["encoder_padding_mask"]
+        self.cache.enc_pad.fill_(1)
+        pad_rows = pm[0].to(torch.uint8) if len(pm) > 0 and pm[0] is not None else 0
+        self.cache.enc_pad.view(B, self.K, self.S)[:, :, :S] = pad_rows[:, None] if torch.is_tensor(pad_rows) else 0
+        for li, layer in enumerate(self.m.decoder.layers):
+            ca = layer.encoder_attn
+            self.cache.cross[li][:, :S] = ops.linear(enc, (ca.k_proj.weight, ca.v_proj.weight),
+                                                     (ca.k_proj.bias, ca.v_proj.bias))
+        self.mask.zero_()
+        self.mask[pad] = -math.inf
+        self.mask[unk] -= unk_penalty
+        self.mask[blank] = -math.inf
+        if mask_idx is not None and mask_idx != unk:
+            self.mask[mask_idx] = -math.inf
+        consts = (int(eos), 1.0 / float(temperature), bool(normalize_scores), float(len_penalty))
+        if self.graphs and consts != self.consts:
+            self.graphs = {}
+        self.consts = consts
+        st = self.state
+        self.min_len.fill_(int(min_len))
+        st["max_len"].fill_(int(max_len))
+        for n in ("lin", "tok", "score", "ignore", "finished", "parent", "cur_score", "fin_n", "stop", "t"):
+            st[n].zero_()
+        st["lin"][:, 0] = torch.arange(self.B * self.K, dtype=torch.int32, device=self.dev)
+        st["cur_tok"].fill_(eos)
+
+    def _body(self, span):
+        m, pre, st = self.m, self.m.text_decoder_prenet, self.state
+        eos, inv_temp, normalize, len_penalty = self.consts
+        BK = self.B * self.K
+        x = ops.scaled_posenc(self.pe.index_select(0, self.t), pre._unit, 0.0, tokens=st["cur_tok"].view(BK, 1),
+                              emb=pre.embed_tokens.weight, padding_idx=pre.padding_idx)
+        self_pad = (self.pos[:span] > self.t).to(torch.uint8)[None].expand(BK, span).contiguous()
+        z, _ = decoder_step(m.decoder, x, self.cache, t_dev=self.t, span=span, self_pad=self_pad, self_rows=st["lin"],
+                            cross_div=self.K)
+        logits = m.text_decoder_postnet(z)
+        kernels.beam_topk(logits[:, -1, :], st["cur_score"], self.mask, inv_temp, eos, self.t, self.min_len,
+                          st["max_len"], st["cand_score"], st["cand_token"], st["cand_beam"], K=self.K)
+        kernels.beam_update(st, K=self.K, V=self.V, eos=eos, normalize=normalize, len_penalty=len_penalty)
+        self.t += 1
+
+    _span = SynthesisGraph._span
+    run = SynthesisGraph.run
+
+    def _snapshot(self):
+        names = ("lin", "ignore", "finished", "cur_tok", "cur_score", "fin_n")
+        keep = {n: self.state[n].clone() for n in names}
+
+        def undo():  # (the lineage gather and the finalized counts are read-modify-write; the rest is rewritten)
+            for n in names:
+                self.state[n].copy_(keep[n])
+        return undo
+
+    @torch.no_grad()
+    def decode(self, encoder_out, max_len, **kw):
+        """Returns SequenceGenerator's hypotheses: per sentence, a list of its finalized hypotheses sorted by score
+        descending (sequence_generator.py:644-654), each {"tokens", "score", "attention": None, "alignment",
+        "positional_scores"}."""
+        self.begin(encoder_out, max_len, **kw)
+        idx = 0
+        while idx <= max_len:
+            n = min(self.CHUNK, max_len + 1 - idx)
+            flags = self.run(idx, n)
+            idx += n
+            if any(flags):
+                break
+        st = self.state
+        fin_n, fin_len = st["fin_n"].tolist(), st["fin_len"].tolist()
+        fin_score, fin_tok, fin_pos = st["fin_score"].cpu(), st["fin_tok"].cpu(), st["fin_pos"].cpu()
+        out = []
+        for s in range(self.B):
+            hyps = [{"tokens": fin_tok[s, i, :fin_len[s][i]].long().to(self.dev), "score": fin_score[s, i].to(self.dev),
+                     "attention": None, "alignment": torch.empty(0),
+                     "positional_scores": fin_pos[s, i, :fin_len[s][i]].to(self.dev)} for i in range(fin_n[s])]
+            order = sorted(range(len(hyps)), key=lambda i: -float(fin_score[s, i]))
+            out.append([hyps[i] for i in order])
+        return out
+
+
+def beam_graph(model, B, K, S, max_len, device, capture=True):
+    """The model's BeamGraph for B sentences x K beams, encoder length S and max_len steps (buckets: S to multiples of
+    64, max_len to powers of two >= 64); rebuilt when the numeric mode or the weights changed."""
+    S_b = max(64, (S + 63) // 64 * 64)
+    M_b = 64
+    while M_b < max_len:
+        M_b *= 2
+    store = model.__dict__.setdefault("_beam_graphs", {})
+    key = (B, K, S_b, M_b, RT.dtype, str(device), bool(capture), RT.param_epoch)
+    bg = store.get(key)
+    if bg is None:
+        for k in [k for k in store if k[:7] == key[:7]]:
+            del store[k]
+        bg = store[key] = BeamGraph(model, B, K, S_b, M_b, device, capture=capture)
+    return bg

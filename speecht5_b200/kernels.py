@@ -217,6 +217,59 @@ def attn_decode_fwd(q, k, v, out, *, H, scale, key_pad=None, probs=None):
     _count(1 if nws == 0 else 2)
 
 
+def attn_lineage_fwd(q, k, v, out, *, H, scale, key_pad=None, kv_rows=None, kv_div=1):
+    """st5_attn_lineage_fwd (include/speecht5_b200.h): attn_decode_fwd for B query rows q [B, 1, H*64] whose key /
+    value j lives in batch row kv_rows[b, j] (int32 [B, >= Tk]) of k / v [*, Tk, H*64], or in row b // kv_div."""
+    _require_cuda(q, k, v, out, key_pad, kv_rows)
+    assert q.dtype == k.dtype == v.dtype == out.dtype and k.stride(2) == 1 and v.stride(2) == 1
+    B, Tk = q.shape[0], k.shape[1]
+    assert kv_rows is None or (kv_rows.dtype == torch.int32 and kv_rows.stride(1) == 1 and kv_rows.shape[0] == B)
+    lib = _lib.load()
+    nws = lib.st5_attn_decode_ws_floats(B, H, Tk, 0)
+    ws = torch.empty(nws, dtype=torch.float32, device=out.device) if nws > 0 else None
+    a = _lib.AttnLineageArgs()
+    d = a.base
+    d.B, d.H, d.Tk, d.dtype = B, H, Tk, dtype_id(out)
+    d.q, d.q_bs = q.data_ptr(), q.stride(0)
+    d.k, d.k_ld, d.k_bs = k.data_ptr(), k.stride(1), k.stride(0)
+    d.v, d.v_ld, d.v_bs = v.data_ptr(), v.stride(1), v.stride(0)
+    d.key_pad, d.out, d.o_bs, d.probs = _ptr(key_pad), out.data_ptr(), out.stride(0), None
+    d.scale, d.ws = scale, _ptr(ws)
+    a.kv_rows, a.kv_rows_ld, a.kv_div = _ptr(kv_rows), (kv_rows.stride(0) if kv_rows is not None else 0), kv_div
+    _lib.check(lib.st5_attn_lineage_fwd(C.byref(a), _stream()), "st5_attn_lineage_fwd")
+    _count(1 if nws == 0 else 2)
+
+
+def beam_topk(logits, cum, mask, inv_temp, eos, t, min_len, max_len, cand_score, cand_token, cand_beam, *, K):
+    """st5_beam_topk: logits [B*K, V] (row pitch logits.stride(0), fp32 / bf16), cum [B*K] fp32, mask [V] fp32; t /
+    min_len / max_len int64 device scalars; cand_* [B, 2K] (fp32, int32, int32) receive the first min(2K, F-1)."""
+    _require_cuda(logits, cum, mask, t, min_len, max_len, cand_score, cand_token, cand_beam)
+    assert logits.stride(1) == 1 and cum.dtype == torch.float32 and mask.dtype == torch.float32
+    assert t.dtype == min_len.dtype == max_len.dtype == torch.int64
+    assert cand_score.dtype == torch.float32 and cand_token.dtype == cand_beam.dtype == torch.int32
+    BK, V = logits.shape
+    B = BK // K
+    lib = _lib.load()
+    ws = torch.empty(max(1, lib.st5_beam_topk_ws_floats(B, K)), dtype=torch.float32, device=logits.device)
+    _lib.check(lib.st5_beam_topk(_ptr(logits), logits.stride(0), dtype_id(logits), B, K, V, _ptr(cum), _ptr(mask),
+                                 float(inv_temp), int(eos), _ptr(t), _ptr(min_len), _ptr(max_len), _ptr(cand_score),
+                                 _ptr(cand_token), _ptr(cand_beam), _ptr(ws), _stream()), "st5_beam_topk")
+    _count(2)
+
+
+def beam_update(st, *, K, V, eos, normalize, len_penalty):
+    """st5_beam_update on the state dict `st` (speecht5_b200/incremental.BeamGraph.state: the tensors the header names,
+    lin / tok / score / fin_tok / fin_pos [.., T] with T = their last dimension)."""
+    names = ("t", "max_len", "cand_score", "cand_token", "cand_beam", "lin", "tok", "score", "ignore", "finished",
+             "parent", "cur_tok", "cur_score", "fin_n", "fin_tok", "fin_pos", "fin_len", "fin_score", "stop")
+    _require_cuda(*(st[n] for n in names))
+    B, T = st["finished"].shape[0], st["lin"].shape[-1]
+    lib = _lib.load()
+    _lib.check(lib.st5_beam_update(B, K, V, T, int(eos), *(_ptr(st[n]) for n in names[:2]), int(bool(normalize)),
+                                   float(len_penalty), *(_ptr(st[n]) for n in names[2:]), _stream()), "st5_beam_update")
+    _count(2)
+
+
 def attn_bwd(a):
     lib = _lib.load()
     _lib.check(lib.st5_attn_bwd(C.byref(a), _stream()), "st5_attn_bwd")

@@ -1063,13 +1063,23 @@ class AttentionTCFn(torch.autograd.Function):
         return dq_buf, (None if same else dkv_buf), dpe, None, None
 
 
-def attention_decode(q_buf, kv_buf, *, H, d, q_col, k_col, v_col, scale, key_pad=None, return_probs=False):
+def attention_decode(q_buf, kv_buf, *, H, d, q_col, k_col, v_col, scale, key_pad=None, return_probs=False,
+                     kv_rows=None, kv_div=1):
     """One query row per utterance (incremental decoding, forward only) on st5_attn_decode_fwd: q_buf [B, 1, nq*d],
     kv_buf [B, Tk, nk*d] with q / k / v in column blocks q_col / k_col / v_col (kv_buf None: q_buf), key_pad [B, Tk]
-    (nonzero / True = masked). Returns (out [B, 1, d], probs [B, H, 1, Tk] fp32 when return_probs else None)."""
+    (nonzero / True = masked). Returns (out [B, 1, d], probs [B, H, 1, Tk] fp32 when return_probs else None).
+    Beam search (st5_attn_lineage_fwd, no probabilities): kv_rows int32 [B, >= Tk] names the kv_buf row of each key of
+    query row b, or kv_div > 1 makes query row b read kv_buf row b // kv_div."""
     kvb = q_buf if kv_buf is None else kv_buf
-    B, Tk = kvb.shape[0], kvb.shape[1]
+    B, Tk = q_buf.shape[0], kvb.shape[1]
     assert q_buf.shape[1] == 1 and d == H * 64 and q_buf.dtype == kvb.dtype
+    if kv_rows is not None or kv_div != 1:
+        assert not return_probs
+        out = torch.empty((B, 1, d), dtype=q_buf.dtype, device=q_buf.device)
+        K.attn_lineage_fwd(q_buf.narrow(2, q_col * d, d), kvb.narrow(2, k_col * d, d), kvb.narrow(2, v_col * d, d), out,
+                           H=H, scale=scale, key_pad=_key_pad_u8(key_pad), kv_rows=kv_rows, kv_div=kv_div)
+        return out, None
+    assert kvb.shape[0] == B
     out = torch.empty((B, 1, d), dtype=q_buf.dtype, device=q_buf.device)
     probs = torch.empty((B, H, 1, Tk), dtype=torch.float32, device=q_buf.device) if return_probs else None
     K.attn_decode_fwd(q_buf.narrow(2, q_col * d, d), kvb.narrow(2, k_col * d, d), kvb.narrow(2, v_col * d, d), out,
