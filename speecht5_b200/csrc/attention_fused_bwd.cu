@@ -2,14 +2,16 @@
 // exp(s - rowmax) with the dropout decision in the sign bit, normalised here by the saved 1/rowsum -- so one step needs
 // a single score-sized MMA, no exponential and no random numbers.
 //
-// One CTA per (head, utterance). Loop: key block kb (64 keys) outer, query tile qt (64 rows) inner; step it:
-//   MMA warpgroup  dP = dO_qt V_kb^T -> shared memory (fp32 rows)
-//   threads        (4 warps, 1 thread = 1 query row x 32 keys): dS = P * (dP_masked + dP_ext - delta);
-//                  dropout(P) and dS -> shared memory tiles (bf16, 128B-swizzled [q][key])
-//   MMA warpgroup  dV_kb += dropout(P)^T dO_qt, dK_kb += dS^T Q_qt (registers, the tiles read MN-major),
-//                  dQ_qt(kb) = dS K_kb -> fp32 accumulator in HBM straight from the fragments (plain RMW: the CTA owns
-//                  its (b,h)), bf16 on the last key block; dK_kb / dV_kb after the last query tile of the block.
-// Q / dO and the saved exponentials are double buffered: TMA fetches those of step it+1 while step it runs.
+// One CTA per (head, utterance), two MMA warpgroups: in round j, A owns key block 2j and B key block 2j+1 (dK / dV in
+// registers); both walk the query tiles qt (64 rows; causal: from qt = 2j) over one shared Q / dO tile per step:
+//   each warpgroup  dP = dO_qt V_kb^T (registers); on the fragments: dS = P * (dP_masked + dP_ext - delta) and
+//                   dropout(P) -> its shared memory tiles (bf16, 128B-swizzled [q][key]);
+//                   dQ_qt(kb) = dS K_kb, then dV_kb += dropout(P)^T dO_qt, dK_kb += dS^T Q_qt (tiles read MN-major).
+//   dQ_qt          running fp32 sum over the key blocks in ascending order: A adds block 2j to the sum of the blocks
+//                   before it (prefetched from the dq_acc scratch by the producer warp a step ahead), B adds 2j+1 and
+//                   stores the sum back to dq_acc -- bf16 into dq after the last block that reaches the tile.
+// While one warpgroup forms dS the other's MMAs run. Q / dO / the saved exponentials and the prefetched running sum
+// are double buffered per step, K / V per round.
 // Semantics: backward of speecht5/models/modules/multihead_attention.py:340-389. With relative positions the two table
 // contractions dQ += dQP PE and dPE = dQP^T Q run on the batched GEMM from the dS written here.
 #include "../../include/speecht5_b200.h"
@@ -22,10 +24,9 @@ namespace st5 {
 int set_error(int code, const char* where);
 
 constexpr int FB_T = 64;                 // query tile == key block
-constexpr int FB_THREADS = 9 * 32;       // MMA warpgroup, TMA warp, 4 compute warps
-constexpr int FB_DPP = FB_T + 4;         // floats per row of the dP tile (row-per-lane float4 reads: conflict-free)
-// K V | Q x2 | dO x2 | dropout(P) x2 | dS | dP | barriers
-constexpr size_t FB_SMEM = 2 * 8192 + 4 * 8192 + 2 * 8192 + 8192 + (size_t)FB_T * FB_DPP * 4 + 256 + 1024;
+constexpr int FB_THREADS = 9 * 32;       // MMA warpgroups A and B, TMA / prefetch warp
+// K V x2 x2 | Q x2 | dO x2 | dropout(P) x2 x2 | dS x2 | dQ running sum x2 | dQ handoff | barriers
+constexpr size_t FB_SMEM = 8 * 8192 + 2 * 8192 + 2 * 8192 + 4 * 8192 + 2 * 8192 + 2 * 16384 + 16384 + 256 + 1024;
 
 struct FusedBwdParams {
   int B, H, Tq, Tk, causal;
@@ -126,268 +127,299 @@ __global__ void attn_delta_ext_kernel(const float* __restrict__ probs, const flo
   if (lane == 0) delta[row] += acc;
 }
 
+// named barrier of one warpgroup (ids 1 and 2; 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar_sync(int g) {
+  if (g == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+  else asm volatile("bar.sync 2, 128;" ::: "memory");
+}
+__device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_release_add(uint32_t* p, uint32_t v) {
+  asm volatile("red.release.cta.shared::cta.add.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
+}
+__device__ __forceinline__ void cp_async8(void* dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+// the barrier receives this thread's arrival once all of its earlier cp.async copies have landed
+__device__ __forceinline__ void cp_async_arrive(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
 __global__ void __launch_bounds__(FB_THREADS, 1)
     attn_fused_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                           const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do,
                           const __grid_constant__ CUtensorMap map_p, const FusedBwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sK = smem;             // [64 keys][128 B]
-  uint8_t* sV = sK + 8192;
-  uint8_t* sQ = sV + 8192;        // 2 x [64 rows][128 B]
-  uint8_t* sdO = sQ + 16384;      // 2 x [64 rows][128 B]
-  uint8_t* sPd = sdO + 16384;     // 2 x [64 rows][64 keys]: the saved exponentials, overwritten in place by dropout(P)
-  uint8_t* sdS = sPd + 16384;     // [64 rows][64 keys]
-  float* sDP = reinterpret_cast<float*>(sdS + 8192);  // [64][FB_DPP]
-  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sDP + FB_T * FB_DPP);  // K/V of a key block landed
-  uint64_t* bar_kvfree = bar_kv + 1;  // every MMA that reads this key block's K/V tiles has completed
-  uint64_t* bar_qdo = bar_kv + 2;     // [2] Q/dO buffer filled
-  uint64_t* bar_qfree = bar_kv + 4;   // [2] Q/dO/exponential buffers consumed by the step's MMAs
-  uint64_t* bar_pin = bar_kv + 6;     // [2] the saved exponentials of a step have landed in sPd[buf] (TMA)
-  uint64_t* bar_dp = bar_kv + 8;      // dP of the step is in sDP
-  uint64_t* bar_pds = bar_kv + 9;     // threads: dropout(P)/dS tiles written, dP read
+  uint8_t* sK = smem;             // [round buffer][warpgroup] x [64 keys][128 B]
+  uint8_t* sV = sK + 4 * 8192;
+  uint8_t* sQ = sV + 4 * 8192;    // [step buffer] x [64 rows][128 B]
+  uint8_t* sdO = sQ + 2 * 8192;
+  uint8_t* sP = sdO + 2 * 8192;   // [step buffer][warpgroup] x [64 rows][64 keys]: exponentials, overwritten by dropout(P)
+  uint8_t* sdS = sP + 4 * 8192;   // [warpgroup] x [64 rows][64 keys]
+  float2* sAcc = reinterpret_cast<float2*>(sdS + 2 * 8192);  // [step buffer] x [16][128]: dQ running sum, fragment order
+  float2* sX = sAcc + 2 * 2048;                              // [16][128]: warpgroup A's partial dQ sum for B
+  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sX + 2048);  // [2] K/V of a round landed
+  uint64_t* bar_kvfree = bar_kv + 2;   // [2] both warpgroups are done with a round's K/V buffer
+  uint64_t* bar_qdo = bar_kv + 4;      // [2] Q, dO and both exponential tiles of a step landed
+  uint64_t* bar_qfree = bar_kv + 6;    // [2] both warpgroups' MMAs of the step have completed
+  uint64_t* bar_acc = bar_kv + 8;      // [2] dQ running sum of the step is in sAcc
+  uint64_t* bar_accfree = bar_kv + 10; // [2] warpgroup A has read sAcc
+  uint64_t* bar_x = bar_kv + 12;       // sX written by A
+  uint64_t* bar_xfree = bar_kv + 13;   // sX read by B
+  uint32_t* acc_done = reinterpret_cast<uint32_t*>(bar_kv + 14);  // 4 x steps B has finished (dq_acc stored)
 
   const int warp = threadIdx.x >> 5;
   const int h = blockIdx.x, b = blockIdx.y;
   const int nkb = (p.Tk + FB_T - 1) / FB_T, nqt = (p.Tq + FB_T - 1) / FB_T;
 
-  if (warp == 4 && elect_one()) {
+  if (warp == 8 && elect_one()) {
     tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); tma_prefetch_desc(&map_do);
     tma_prefetch_desc(&map_p);
-    mbar_init(bar_kv, 1); mbar_init(bar_kvfree, 1);
     for (int s = 0; s < 2; ++s) {
-      mbar_init(&bar_qdo[s], 1); mbar_init(&bar_qfree[s], 1); mbar_init(&bar_pin[s], 1);
+      mbar_init(&bar_kv[s], 1); mbar_init(&bar_kvfree[s], 2);
+      mbar_init(&bar_qdo[s], 1); mbar_init(&bar_qfree[s], 2);
+      mbar_init(&bar_acc[s], 32); mbar_init(&bar_accfree[s], 128);
     }
-    mbar_init(bar_dp, 128);
-    mbar_init(bar_pds, 4);
+    mbar_init(bar_x, 128); mbar_init(bar_xfree, 128);
+    *acc_done = 0u;
     fence_mbar_init();
   }
   __syncthreads();
   pdl_sync();  // (prologue done: nothing above touched global memory)
 
-  if (warp == 4) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      int it = 0, kbc = 0;
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int qt0 = p.causal ? kb : 0;
-        for (int qt = qt0; qt < nqt; ++qt, ++it) {
-          const int buf = it & 1;
-          if (qt == qt0) {
-            if (kbc > 0) mbar_wait_quiet(bar_kvfree, (uint32_t)((kbc - 1) & 1));  // MMAs of the previous key block are done
-            ++kbc;
-            mbar_expect_tx(bar_kv, 16384);
-            tma_load_4d(sK, &map_k, bar_kv, 0, kb * FB_T, h, b);
-            tma_load_4d(sV, &map_v, bar_kv, 0, kb * FB_T, h, b);
-          }
-          if (it >= 2) mbar_wait_quiet(&bar_qfree[buf], (uint32_t)(((it >> 1) - 1) & 1));  // step it-2 has read this buffer
-          mbar_expect_tx(&bar_qdo[buf], 16384);
-          tma_load_4d(sQ + buf * 8192, &map_q, &bar_qdo[buf], 0, qt * FB_T, h, b);
-          tma_load_4d(sdO + buf * 8192, &map_do, &bar_qdo[buf], 0, qt * FB_T, h, b);
-          // the saved exponentials of this (query tile, key block) go straight into the operand tile the threads will
-          // overwrite in place with dropout(P): [64 rows][64 keys], 128B-swizzled
-          mbar_expect_tx(&bar_pin[buf], 8192u);
-          tma_load_4d(sPd + buf * 8192, &map_p, &bar_pin[buf], kb * FB_T, qt * FB_T, h, b);
+  if (warp == 8) {
+    // ===================== TMA producer + dQ running-sum prefetch =====================
+    const int lane = (int)lane_id();
+    int s = 0, rc = 0;
+    for (int j = 0; 2 * j < nkb; ++j) {
+      const int qt0 = p.causal ? 2 * j : 0;
+      if (qt0 >= nqt) break;  // causal, Tk > Tq: no later round has a step either
+      const bool hasB = 2 * j + 1 < nkb;
+      const int kbuf = rc & 1;
+      if (lane == 0) {
+        if (rc >= 2) mbar_wait_quiet(&bar_kvfree[kbuf], (uint32_t)(((rc >> 1) - 1) & 1));
+        mbar_expect_tx(&bar_kv[kbuf], hasB ? 32768u : 16384u);
+        tma_load_4d(sK + (2 * kbuf) * 8192, &map_k, &bar_kv[kbuf], 0, 2 * j * FB_T, h, b);
+        tma_load_4d(sV + (2 * kbuf) * 8192, &map_v, &bar_kv[kbuf], 0, 2 * j * FB_T, h, b);
+        if (hasB) {
+          tma_load_4d(sK + (2 * kbuf + 1) * 8192, &map_k, &bar_kv[kbuf], 0, (2 * j + 1) * FB_T, h, b);
+          tma_load_4d(sV + (2 * kbuf + 1) * 8192, &map_v, &bar_kv[kbuf], 0, (2 * j + 1) * FB_T, h, b);
         }
       }
+      ++rc;
+      for (int qt = qt0; qt < nqt; ++qt, ++s) {
+        const int buf = s & 1;
+        const bool bOn = hasB && (!p.causal || qt > 2 * j);  // key block 2j+1 reaches this query tile
+        if (lane == 0) {
+          if (s >= 2) mbar_wait_quiet(&bar_qfree[buf], (uint32_t)(((s >> 1) - 1) & 1));  // step s-2 is done with it
+          mbar_expect_tx(&bar_qdo[buf], bOn ? 32768u : 24576u);
+          tma_load_4d(sQ + buf * 8192, &map_q, &bar_qdo[buf], 0, qt * FB_T, h, b);
+          tma_load_4d(sdO + buf * 8192, &map_do, &bar_qdo[buf], 0, qt * FB_T, h, b);
+          tma_load_4d(sP + (2 * buf) * 8192, &map_p, &bar_qdo[buf], 2 * j * FB_T, qt * FB_T, h, b);
+          if (bOn) tma_load_4d(sP + (2 * buf + 1) * 8192, &map_p, &bar_qdo[buf], (2 * j + 1) * FB_T, qt * FB_T, h, b);
+        }
+        __syncwarp();
+        if (s >= 2) mbar_wait_quiet(&bar_accfree[buf], (uint32_t)(((s >> 1) - 1) & 1));
+        if (j > 0) {
+          // The running sum of this tile was stored to dq_acc by warpgroup B in step (j-1, qt), nqt - qt0 steps back:
+          // wait until B has counted that step (release after its stores), then copy the tile in fragment order.
+          const uint32_t need = 4u * (uint32_t)(s - (nqt - qt0) + 1);
+          if (ld_acquire_u32(acc_done) < need) {
+            const long long t0 = clock64();
+            while (ld_acquire_u32(acc_done) < need)
+              if (clock64() - t0 > 4000000000LL) __trap();
+          }
+          float2* dst = sAcc + buf * 2048;
+#pragma unroll 4
+          for (int w = 0; w < 4; ++w)
+#pragma unroll
+            for (int i2 = 0; i2 < 16; ++i2) {
+              const int row = qt * FB_T + 16 * w + (lane >> 2) + 8 * (i2 & 1), col = 8 * (i2 >> 1) + 2 * (lane & 3);
+              if (row < p.Tq)
+                cp_async8(dst + i2 * 128 + w * 32 + lane, p.dq_acc + ((int64_t)b * p.Tq + row) * (p.H * 64) + h * 64 + col);
+            }
+        }
+        cp_async_arrive(&bar_acc[buf]);
+      }
     }
-  } else if (warp < 4) {
-    // ===================== MMA warpgroup =====================
-    const uint32_t aK = smem_u32(sK), aV = smem_u32(sV), aQ0 = smem_u32(sQ), adO0 = smem_u32(sdO);
-    const uint32_t aPd0 = smem_u32(sPd), adS = smem_u32(sdS);
-    const int l = (int)lane_id(), w = warp;
+    asm volatile("cp.async.wait_all;" ::: "memory");
+  } else {
+    // ===================== MMA warpgroups: A (g = 0) even key blocks, B (g = 1) odd ones =====================
+    const int g = warp >> 2;
+    const int tid = threadIdx.x & 127;
+    const int l = (int)lane_id(), w = warp & 3;
     const int r0 = 16 * w + (l >> 2);  // fragment rows r0, r0 + 8; columns 8 (i >> 2) + 2 (l & 3) + (i & 1)
+    const uint32_t aQ0 = smem_u32(sQ), adO0 = smem_u32(sdO), adS = smem_u32(sdS + g * 8192);
+    uint8_t* tS = sdS + g * 8192;
     float dk[32], dv[32];
 #pragma unroll
     for (int t = 0; t < 32; ++t) dk[t] = dv[t] = 0.f;
-    int it = 0, kbc = 0;
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int qt0 = p.causal ? kb : 0;
-      if (qt0 >= nqt) {  // causal, Tk > Tq: no query row sees the keys of this block, their gradients are zero
+    int s = 0, rc = 0, nx = 0;
+    for (int j = 0; 2 * j < nkb; ++j) {
+      const int kb = 2 * j + g;
+      const int qt0 = p.causal ? 2 * j : 0;
+      const int qtm = p.causal ? kb : 0;  // first query tile this warpgroup's key block reaches
+      const bool active = kb < nkb && qtm < nqt;
+      if (qt0 < nqt) {
+        const int kbuf = rc & 1;
+        if (active) mbar_wait_quiet(&bar_kv[kbuf], (uint32_t)((rc >> 1) & 1));
+        ++rc;
+        const uint32_t aK = smem_u32(sK + (2 * kbuf + g) * 8192), aV = smem_u32(sV + (2 * kbuf + g) * 8192);
+        for (int qt = qt0; qt < nqt; ++qt, ++s) {
+          const int buf = s & 1;
+          if (kb < nkb && qt >= qtm) {
+            const uint32_t aQ = aQ0 + (uint32_t)buf * 8192u, adO = adO0 + (uint32_t)buf * 8192u;
+            uint8_t* tP = sP + (2 * buf + g) * 8192;
+            const uint32_t aP = smem_u32(tP);
+            const int i0 = qt * FB_T + r0;
+            const bool ok0 = i0 < p.Tq, ok1 = i0 + 8 < p.Tq;
+            const int64_t prow0 = ((int64_t)b * p.H + h) * p.Tq + i0;
+            const float invl0 = ok0 ? p.inv_l[prow0] : 0.f, delta0 = ok0 ? p.delta[prow0] : 0.f;
+            const float invl1 = ok1 ? p.inv_l[prow0 + 8] : 0.f, delta1 = ok1 ? p.delta[prow0 + 8] : 0.f;
+            mbar_wait_quiet(&bar_qdo[buf], (uint32_t)((s >> 1) & 1));
+            float dp[32];
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k)  // dP = dO V^T (A = dO, B = V: both K-major over the head dimension)
+              wgmma_m64n64<0, 0>(dp, wgmma_smem_desc(adO + k * 32, 16, 1024), wgmma_smem_desc(aV + k * 32, 16, 1024),
+                                 k != 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(dp);
+            // ---- softmax gradient on the fragment: dropout(P) in place of the exponentials, dS into its own tile.
+            // Rows beyond Tq / keys beyond Tk in a live 32 x 32 quadrant compute to zero (their exponentials, dO and
+            // V rows arrive as zeros); a quadrant with no live row or key is written as +0 without being read.
+            const bool rows_dead = qt * FB_T + (w >= 2 ? 32 : 0) >= p.Tq;
+            const bool ext = p.dp_ext != nullptr && h < p.ext_heads;
+            const float* dpx0 = ext && ok0 ? p.dp_ext + prow0 * p.p_ld : nullptr;
+            const float* dpx1 = ext && ok1 ? p.dp_ext + (prow0 + 8) * p.p_ld : nullptr;
+            const bool x_vec = (reinterpret_cast<uintptr_t>(p.dp_ext) & 7) == 0;
+#pragma unroll
+            for (int i = 0; i < 32; i += 2) {
+              const int hr = (i >> 1) & 1;
+              const int rr = r0 + 8 * hr, key = kb * FB_T + 8 * (i >> 2) + 2 * (l & 3);
+              const int off = rr * 128 + ((((i >> 2) ^ (l >> 2)) << 4) | ((l & 3) << 2));  // 128B swizzle
+              uint32_t pdw = 0u, dsw = 0u;
+              if (!rows_dead && kb * FB_T + (i >= 16 ? 32 : 0) < p.Tk) {
+                const uint32_t e2 = *reinterpret_cast<const uint32_t*>(tP + off);  // two saved exponentials
+                const float* dpx = hr ? dpx1 : dpx0;
+                float xd0 = 0.f, xd1 = 0.f;
+                if (dpx != nullptr) {  // the caller's gradient on the probabilities (keys < Tk only)
+                  if (x_vec && key + 1 < p.Tk) {
+                    const float2 x = __ldg(reinterpret_cast<const float2*>(dpx + key));
+                    xd0 = x.x; xd1 = x.y;
+                  } else {
+                    if (key < p.Tk) xd0 = dpx[key];
+                    if (key + 1 < p.Tk) xd1 = dpx[key + 1];
+                  }
+                }
+                const float invl = hr ? invl1 : invl0, delta = hr ? delta1 : delta0;
+                const uint32_t raw0 = e2 << 16, raw1 = e2 & 0xffff0000u;  // bf16 -> fp32 bit patterns
+                const float keep0 = (int32_t)raw0 < 0 ? 0.f : p.drop_scale;  // sign bit = dropped by the forward pass
+                const float keep1 = (int32_t)raw1 < 0 ? 0.f : p.drop_scale;
+                const float pv0 = fabsf(__uint_as_float(raw0)) * invl, pv1 = fabsf(__uint_as_float(raw1)) * invl;
+                // dP as the softmax sees it: dropout backward of dO V^T, plus the caller's gradient
+                const float dp0 = dp[i] * keep0 + xd0, dp1 = dp[i + 1] * keep1 + xd1;
+                pdw = pack2(pv0 * keep0, pv1 * keep1);
+                dsw = pack2(pv0 * (dp0 - delta), pv1 * (dp1 - delta));
+              }
+              *reinterpret_cast<uint32_t*>(tP + off) = pdw;
+              *reinterpret_cast<uint32_t*>(tS + off) = dsw;
+              if (p.ds_out != nullptr && (hr ? ok1 : ok0) && key < p.p_ld)
+                *reinterpret_cast<uint32_t*>(p.ds_out + (prow0 + 8 * hr) * p.p_ld + key) = dsw;
+            }
+            fence_proxy_async();
+            wg_bar_sync(g);  // the whole warpgroup's tiles are written before its MMAs read them
+            float dq[32];
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k)  // contraction over the 64 keys: A = dS (K-major), B = K (MN-major)
+              wgmma_m64n64<0, 1>(dq, wgmma_smem_desc(adS + k * 32, 16, 1024), wgmma_smem_desc(aK + k * 2048, 8192, 1024),
+                                 k != 0 ? 1u : 0u);
+            wgmma_commit();
+            const uint32_t acc = qt != qtm;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {  // contraction over the 64 query rows: A = P^T / dS^T, B = dO / Q (MN-major)
+              wgmma_m64n64<1, 1>(dv, wgmma_smem_desc(aP + k * 2048, 8192, 1024), wgmma_smem_desc(adO + k * 2048, 8192, 1024),
+                                 acc | (uint32_t)(k != 0));
+              wgmma_m64n64<1, 1>(dk, wgmma_smem_desc(adS + k * 2048, 8192, 1024), wgmma_smem_desc(aQ + k * 2048, 8192, 1024),
+                                 acc | (uint32_t)(k != 0));
+            }
+            wgmma_commit();
+            wgmma_wait<1>();  // dQ is ready; dV / dK keep the tensor pipe busy meanwhile
+            wgmma_fence_regs(dq);
+            // ---- dQ of (kb, qt): running fp32 sum over the key blocks in ascending order, bf16 after the last one.
+            // A adds the sum of blocks < 2j (prefetched) and hands it to B, which adds block 2j+1 and stores it --
+            // unless 2j is the last block that reaches the tile, then A stores.
+            const int kb_last = p.causal ? (qt < nkb - 1 ? qt : nkb - 1) : nkb - 1;
+            const bool last = kb == kb_last;
+            const float2* src;
+            if (g == 0) {
+              mbar_wait_quiet(&bar_acc[buf], (uint32_t)((s >> 1) & 1));
+              src = sAcc + buf * 2048 + tid;
+              if (!last && nx > 0) mbar_wait_quiet(bar_xfree, (uint32_t)((nx - 1) & 1));
+            } else {
+              mbar_wait_quiet(bar_x, (uint32_t)(nx & 1));
+              src = sX + tid;
+            }
+            const bool add = g == 1 || kb > 0;
+            const bool keep = g == 0 && !last;
+#pragma unroll
+            for (int i = 0; i < 32; i += 2) {
+              const int row = qt * FB_T + r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
+              float2 f = make_float2(dq[i] * p.scale, dq[i + 1] * p.scale);
+              if (add) {
+                const float2 o = src[(i >> 1) * 128];
+                f.x += o.x; f.y += o.y;
+              }
+              if (keep) {
+                sX[(i >> 1) * 128 + tid] = f;
+              } else if (row < p.Tq) {
+                if (last)
+                  *reinterpret_cast<uint32_t*>(p.dq + (int64_t)b * p.q_bs + (int64_t)row * p.q_ld + h * 64 + col) =
+                      pack2(f.x, f.y);
+                else
+                  *reinterpret_cast<float2*>(p.dq_acc + ((int64_t)b * p.Tq + row) * (p.H * 64) + h * 64 + col) = f;
+              }
+            }
+            if (g == 0) {
+              mbar_arrive(&bar_accfree[buf]);
+              if (!last) { mbar_arrive(bar_x); ++nx; }
+            } else {
+              mbar_arrive(bar_xfree); ++nx;
+            }
+            wgmma_wait<0>();
+            wgmma_fence_regs(dk);
+            wgmma_fence_regs(dv);
+          } else {
+            // B without a block for this tile still releases the step: not before the step's tiles have landed,
+            // i.e. after step s-2 was released by both warpgroups -- its arrival must not complete an earlier phase
+            mbar_wait_quiet(&bar_qdo[buf], (uint32_t)((s >> 1) & 1));
+          }
+          if (tid == 0) mbar_arrive(&bar_qfree[buf]);
+          if (g == 1) {  // publish this step's dq_acc stores to the prefetching warp
+            __threadfence_block();
+            __syncwarp();
+            if (l == 0) red_release_add(acc_done, 1u);
+          }
+        }
+        if (tid == 0) mbar_arrive(&bar_kvfree[kbuf]);
+      }
+      if (kb < nkb) {  // dK / dV of the key block (zero when no query row sees it: causal, Tk > Tq)
 #pragma unroll
         for (int i = 0; i < 32; i += 2) {
           const int key = kb * FB_T + r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
           if (key < p.Tk) {
-            *reinterpret_cast<uint32_t*>(p.dk + (int64_t)b * p.k_bs + (int64_t)key * p.k_ld + h * 64 + col) = 0u;
-            *reinterpret_cast<uint32_t*>(p.dv + (int64_t)b * p.v_bs + (int64_t)key * p.v_ld + h * 64 + col) = 0u;
+            *reinterpret_cast<uint32_t*>(p.dk + (int64_t)b * p.k_bs + (int64_t)key * p.k_ld + h * 64 + col) =
+                active ? pack2(dk[i] * p.scale, dk[i + 1] * p.scale) : 0u;
+            *reinterpret_cast<uint32_t*>(p.dv + (int64_t)b * p.v_bs + (int64_t)key * p.v_ld + h * 64 + col) =
+                active ? pack2(dv[i], dv[i + 1]) : 0u;
           }
         }
-        continue;
-      }
-      mbar_wait_quiet(bar_kv, (uint32_t)(kbc & 1));
-      ++kbc;
-      for (int qt = qt0; qt < nqt; ++qt, ++it) {
-        const int buf = it & 1;
-        const uint32_t aQ = aQ0 + (uint32_t)buf * 8192u, adO = adO0 + (uint32_t)buf * 8192u;
-        const uint32_t aPd = aPd0 + (uint32_t)buf * 8192u;
-        mbar_wait_quiet(&bar_qdo[buf], (uint32_t)((it >> 1) & 1));
-        {  // dP = dO V^T (A = dO, B = V: both K-major over the head dimension)
-          float dp[32];
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            wgmma_m64n64<0, 0>(dp, wgmma_smem_desc(adO + k * 32, 16, 1024), wgmma_smem_desc(aV + k * 32, 16, 1024),
-                               k != 0 ? 1u : 0u);
-          wgmma_commit();
-          wgmma_wait<0>();
-          wgmma_fence_regs(dp);
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const int rr = r0 + 8 * ((i >> 1) & 1), cc = 8 * (i >> 2) + 2 * (l & 3);
-            *reinterpret_cast<float2*>(sDP + rr * FB_DPP + cc) = make_float2(dp[i], dp[i + 1]);
-          }
-        }
-        mbar_arrive(bar_dp);
-        mbar_wait_quiet(bar_pds, (uint32_t)(it & 1));
-        float dq[32];
-        wgmma_fence();
-        const uint32_t acc = qt != qt0;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {  // contraction over the 64 query rows: A = P^T / dS^T, B = dO / Q (all MN-major)
-          wgmma_m64n64<1, 1>(dv, wgmma_smem_desc(aPd + k * 2048, 8192, 1024), wgmma_smem_desc(adO + k * 2048, 8192, 1024),
-                             acc | (uint32_t)(k != 0));
-          wgmma_m64n64<1, 1>(dk, wgmma_smem_desc(adS + k * 2048, 8192, 1024), wgmma_smem_desc(aQ + k * 2048, 8192, 1024),
-                             acc | (uint32_t)(k != 0));
-        }
-#pragma unroll
-        for (int k = 0; k < 4; ++k)  // contraction over the 64 keys: A = dS (K-major), B = K (MN-major)
-          wgmma_m64n64<0, 1>(dq, wgmma_smem_desc(adS + k * 32, 16, 1024), wgmma_smem_desc(aK + k * 2048, 8192, 1024),
-                             k != 0 ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(dq);
-        wgmma_fence_regs(dk);
-        wgmma_fence_regs(dv);
-        if (threadIdx.x == 0) {
-          mbar_arrive(&bar_qfree[buf]);
-          if (qt == nqt - 1) mbar_arrive(bar_kvfree);
-        }
-        // ---- dQ partial of (kb, qt): running fp32 sum over the key blocks, bf16 after the last one
-        const int kb_last = p.causal ? (qt < nkb - 1 ? qt : nkb - 1) : nkb - 1;
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const int row = qt * FB_T + r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
-          if (row < p.Tq) {
-            float2 f = make_float2(dq[i] * p.scale, dq[i + 1] * p.scale);
-            float* accp = p.dq_acc + ((int64_t)b * p.Tq + row) * (p.H * 64) + h * 64 + col;
-            if (kb > 0) {
-              const float2 o = *reinterpret_cast<const float2*>(accp);
-              f.x += o.x; f.y += o.y;
-            }
-            if (kb == kb_last)
-              *reinterpret_cast<uint32_t*>(p.dq + (int64_t)b * p.q_bs + (int64_t)row * p.q_ld + h * 64 + col) = pack2(f.x, f.y);
-            else
-              *reinterpret_cast<float2*>(accp) = f;
-          }
-        }
-        if (qt == nqt - 1) {  // dK / dV of the key block
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const int key = kb * FB_T + r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
-            if (key < p.Tk) {
-              *reinterpret_cast<uint32_t*>(p.dk + (int64_t)b * p.k_bs + (int64_t)key * p.k_ld + h * 64 + col) =
-                  pack2(dk[i] * p.scale, dk[i + 1] * p.scale);
-              *reinterpret_cast<uint32_t*>(p.dv + (int64_t)b * p.v_bs + (int64_t)key * p.v_ld + h * 64 + col) =
-                  pack2(dv[i], dv[i + 1]);
-            }
-          }
-        }
-      }
-    }
-  } else {
-    // ===================== compute threads (thread = query row x 32-key chunk) =====================
-    const int sw = warp - 5;
-    const int q = sw & 1;
-    const int c = sw >> 1;  // this warp's 32-key chunk of the block
-    const int r = q * 32 + (int)lane_id();
-    const int cbase = c * 4;
-    int it = 0;
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int qt0 = p.causal ? kb : 0;
-      const int k0 = kb * FB_T;
-      for (int qt = qt0; qt < nqt; ++qt, ++it) {
-        const int buf = it & 1;
-        const int i = qt * FB_T + r;
-        const bool row_ok = i < p.Tq;
-        const int64_t prow = ((int64_t)b * p.H + h) * p.Tq + i;
-        const float delta = row_ok ? p.delta[prow] : 0.f, invl = row_ok ? p.inv_l[prow] : 0.f;
-        const float* dpx = (p.dp_ext != nullptr && row_ok && h < p.ext_heads) ? p.dp_ext + prow * p.p_ld : nullptr;
-        const int col0 = k0 + c * 32;
-        mbar_wait_quiet(bar_dp, (uint32_t)(it & 1));
-        mbar_wait_quiet(&bar_pin[buf], (uint32_t)((it >> 1) & 1));  // the exponentials are in sPd[buf] (every warp:
-                                                                    // nobody may write the tile before the TMA has)
-        uint8_t* bp = sPd + buf * 8192 + r * 128;
-        uint8_t* bs = sdS + r * 128;
-        // warp-uniform fast path: no live query row in this warp's 32 rows, or the whole key chunk lies beyond Tk --
-        // P is zero there, so both operand tiles get zeros (they are contracted over, so they must be written)
-        const bool dead = (qt * FB_T + q * 32 >= p.Tq) || (col0 >= p.Tk);
-        if (dead) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            const int swz = ((cbase + g) ^ (r & 7)) << 4;
-            *reinterpret_cast<uint4*>(bp + swz) = make_uint4(0u, 0u, 0u, 0u);
-            *reinterpret_cast<uint4*>(bs + swz) = make_uint4(0u, 0u, 0u, 0u);
-            if (p.ds_out != nullptr && row_ok && col0 + 8 * g + 8 <= p.p_ld)
-              *reinterpret_cast<uint4*>(p.ds_out + prow * p.p_ld + col0 + 8 * g) = make_uint4(0u, 0u, 0u, 0u);
-          }
-        } else {
-        // (dP is finite everywhere: V rows beyond Tk and dO rows beyond Tq arrive as zeros from TMA)
-        float dvv[32];
-        {
-          const float* src = sDP + r * FB_DPP + c * 32;
-#pragma unroll
-          for (int t = 0; t < 32; t += 4) {
-            const float4 f = *reinterpret_cast<const float4*>(src + t);
-            dvv[t] = f.x; dvv[t + 1] = f.y; dvv[t + 2] = f.z; dvv[t + 3] = f.w;
-          }
-        }
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int swz = ((cbase + g) ^ (r & 7)) << 4;
-          const uint4 praw = *reinterpret_cast<const uint4*>(bp + swz);  // this row's 8 saved exponentials (in place)
-          const uint32_t w4[4] = {praw.x, praw.y, praw.z, praw.w};
-          float xd[8];
-          xd[0] = xd[1] = xd[2] = xd[3] = xd[4] = xd[5] = xd[6] = xd[7] = 0.f;
-          if (dpx != nullptr) {  // the caller's gradient on the probabilities: this row's 8 floats of the chunk (keys
-                                 // < Tk only: the padding columns [Tk, p_ld) are not part of the contract)
-            if ((p.p_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(p.dp_ext) & 15) == 0 && col0 + 8 * g + 8 <= p.Tk) {
-              const float4 x0 = __ldg(reinterpret_cast<const float4*>(dpx + col0 + 8 * g));
-              const float4 x1 = __ldg(reinterpret_cast<const float4*>(dpx + col0 + 8 * g + 4));
-              xd[0] = x0.x; xd[1] = x0.y; xd[2] = x0.z; xd[3] = x0.w;
-              xd[4] = x1.x; xd[5] = x1.y; xd[6] = x1.z; xd[7] = x1.w;
-            } else {
-#pragma unroll
-              for (int t = 0; t < 8; ++t)
-                if (col0 + 8 * g + t < p.Tk) xd[t] = dpx[col0 + 8 * g + t];
-            }
-          }
-          float pd8[8], ds8[8];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-              const int t = 2 * e + hh;
-              const uint32_t raw = hh ? (w4[e] & 0xffff0000u) : (w4[e] << 16);  // bf16 -> fp32 bit pattern
-              const float keepf = (int32_t)raw < 0 ? 0.f : p.drop_scale;      // sign bit = dropped by the forward pass
-              const float pv = fabsf(__uint_as_float(raw)) * invl;           // the probability
-              // dP as the softmax sees it: dropout backward of dO V^T, plus the caller's gradient
-              const float dp = dvv[8 * g + t] * keepf + xd[t];
-              pd8[t] = pv * keepf;
-              ds8[t] = pv * (dp - delta);
-            }
-          }
-          uint4 a, d;
-          a.x = pack2(pd8[0], pd8[1]); a.y = pack2(pd8[2], pd8[3]); a.z = pack2(pd8[4], pd8[5]); a.w = pack2(pd8[6], pd8[7]);
-          d.x = pack2(ds8[0], ds8[1]); d.y = pack2(ds8[2], ds8[3]); d.z = pack2(ds8[4], ds8[5]); d.w = pack2(ds8[6], ds8[7]);
-          *reinterpret_cast<uint4*>(bp + swz) = a;
-          *reinterpret_cast<uint4*>(bs + swz) = d;
-          if (p.ds_out != nullptr && row_ok && col0 + 8 * g + 8 <= p.p_ld)
-            *reinterpret_cast<uint4*>(p.ds_out + prow * p.p_ld + col0 + 8 * g) = d;
-        }
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane_id() == 0) mbar_arrive(bar_pds);
       }
     }
   }
