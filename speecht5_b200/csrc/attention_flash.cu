@@ -2,24 +2,29 @@
 // It serves both forward entry points: st5_attn_fused_fwd (Tk <= 320, the relative-position variant without clipping)
 // and st5_attn_flash_fwd (any length); the outputs and the psave / inv_l / out_f32 contract are the same.
 //
-// One CTA = (64 query rows, head, utterance). The keys are walked in blocks of 64; nothing of size Tq x Tk stays on
-// chip. The output accumulator lives in the registers of the MMA warpgroup and is never rescaled: the kernel makes the
-// row maximum FINAL before the first exponential, sweeping the key blocks twice (three times when the caller wants
-// normalised probabilities back) and re-issuing the cheap 64 x 64 x 64 score MMA in every sweep:
+// One CTA = (two 64-row query tiles, head, utterance). The keys are walked in blocks of 64; nothing of size Tq x Tk
+// stays on chip. The output accumulator lives in registers and is never rescaled: the kernel makes the row maximum
+// FINAL before the first exponential, sweeping the key blocks twice (three times when the caller wants normalised
+// probabilities back) and re-issuing the cheap 64 x 64 x 64 score MMA in every sweep:
 //
 //   sweep 0   S_kb = Q K_kb^T (+ bias)  -> running row maximum
-//   sweep 1   S_kb again -> e = exp2(s - max), row sum, dropout, P -> smem (bf16) -> O += P V_kb  (registers)
+//   sweep 1   S_kb again -> e = exp2(s - max), row sum, dropout, P (bf16, registers) -> O += P V_kb
 //             and, for the backward pass, e (bf16, sign bit = dropped) -> psave
 //   sweep 2   (only with `probs`) S_kb again -> e / rowsum -> probabilities
 //   epilogue  O / rowsum -> bf16 out (+ fp32 copy), lse, 1 / rowsum
 //
-// Warps: 0..3 = MMA warpgroup (wgmma; S, QP and the finished O leave through shared memory as fp32 rows), 4 = TMA
-// producer, 5..8 = softmax (thread = one query row, one of the two 32-key chunks of a block).
+// Warps: 0..3 and 4..7 = two MMA warpgroups, one query tile each; 8 = TMA producer. Each warpgroup does its softmax on
+// its own accumulator fragments (a row is spread over one quad of lanes) and feeds P to the P V wgmma as its register
+// A operand, so scores and probabilities never go through shared memory. K and V arrive in a ring of stages that both
+// warpgroups read, so each key block is loaded once per 128 query rows. While one warpgroup forms its exponentials the
+// other's MMAs run. Causal CTAs pair tile n-1-x with tile x, so that every CTA does the same work; otherwise tiles 2x
+// and 2x+1 share a CTA. A lone last tile runs with the second warpgroup idle.
 //
 // Relative positions (encoder.py:40-59, 239-246; multihead_attention.py:346-353) with clipping:
 //   bias[i][j] = q_i . pe[clamp(i - j, -maxpos, maxpos - 1) + maxpos]
-// Per key block the kernel computes QPw = Q PEw^T for the 128-row window PEw of the table this (query tile, key block)
-// pair can reach; every softmax thread reads its row of QPw skewed by the key (clamped at the table ends).
+// Per key block each warpgroup computes QPw = Q PEw^T for the 128-row window PEw of the table its (query tile, key
+// block) pair can reach; the skewed read (row i, key j -> column i - j, clamped at the table ends) needs other lanes'
+// columns, so QPw goes through shared memory, one window per warpgroup.
 // Reference semantics: speecht5/models/modules/multihead_attention.py:340-389.
 #include "../../include/speecht5_b200.h"
 #include "kernels.cuh"
@@ -31,16 +36,19 @@ namespace st5 {
 int set_error(int code, const char* where);
 
 constexpr int FL_T = 64;              // query tile == key block
-constexpr int FL_THREADS = 9 * 32;    // MMA warpgroup, TMA warp, 4 softmax warps
+constexpr int FL_THREADS = 9 * 32;    // two MMA warpgroups, TMA warp
 constexpr int FL_PE_ROWS = 128;       // table rows per window (i - j spans 127 values per tile pair)
-constexpr int FL_SP = FL_T + 4;       // floats per row of the S / O tiles (row-per-lane float4 reads: conflict-free)
 constexpr int FL_QPP = FL_PE_ROWS + 4;
 constexpr int FL_MAX_TK_RESIDENT = 320;
 constexpr int FL_MAX_T_RPE_RESIDENT = 160;
-// Q 8K | K 2 x 8K | V 8K | P 8K | S 17K | O 17K | (PEw 2 x 16K | QPw 33K) | barriers + row reductions | slack
+// K / V ring depth: three stages without relative positions; two with them (a stage also holds both PE windows).
+template <bool RPE> constexpr int fl_stages() { return RPE ? 2 : 3; }
+// one stage: K 8K | V 8K | (PEw of each warpgroup 2 x 16K)
+template <bool RPE> constexpr uint32_t fl_stage_bytes() { return 2 * 8192 + (RPE ? 2 * 16384 : 0); }
+// Q 2 x 8K | stages | (QPw 2 x 33K) | barriers | alignment slack
 template <bool RPE> constexpr size_t fl_smem() {
-  return 8192 + 2 * 8192 + 8192 + 8192 + 2 * (size_t)FL_T * FL_SP * 4 +
-         (RPE ? 2 * 16384 + (size_t)FL_T * FL_QPP * 4 : 0) + 128 + 512 + 1024;
+  return 2 * 8192 + (size_t)fl_stages<RPE>() * fl_stage_bytes<RPE>() + (RPE ? 2 * (size_t)FL_T * FL_QPP * 4 : 0) +
+         128 + 1024;
 }
 
 struct FlashFwdParams {
@@ -69,6 +77,22 @@ __host__ __device__ __forceinline__ int fl_window_row0(int i0, int j0, int maxpo
   if (w < 0) w = 0;
   return w;
 }
+// query tiles of CTA x (tb = -1: none): causal CTAs pair the long tile n-1-x with the short tile x, so that all do the
+// same work and ta is the longer one; otherwise neighbours 2x, 2x+1
+__device__ __forceinline__ void fl_tiles(int x, int nqt, bool causal, int& ta, int& tb) {
+  if (causal) {
+    ta = nqt - 1 - x;
+    tb = x < ta ? x : -1;
+  } else {
+    ta = 2 * x;
+    tb = 2 * x + 1 < nqt ? 2 * x + 1 : -1;
+  }
+}
+__device__ __forceinline__ int fl_tile_nkb(int t, int Tk, bool causal) {
+  int tk = Tk;
+  if (causal && (t + 1) * FL_T < tk) tk = (t + 1) * FL_T;
+  return (tk + FL_T - 1) / FL_T;
+}
 // m64nN accumulator fragment -> fp32 rows in shared memory (pitch in floats)
 template <int NR>
 __device__ __forceinline__ void fl_store_acc(float* dst, int pitch, const float (&d)[NR]) {
@@ -80,344 +104,307 @@ __device__ __forceinline__ void fl_store_acc(float* dst, int pitch, const float 
     *reinterpret_cast<float2*>(dst + r * pitch + c) = make_float2(d[i], d[i + 1]);
   }
 }
+__device__ __forceinline__ void fl_bar_wg(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void fl_fence_u32(uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(a[k][i])::"memory");
+}
+// Dropout keep bits of this thread's 32 accumulator elements of one key block (bit i <-> d[i]), at the element index
+// the row-per-thread kernels use (prow * attn_drop_pitch(Tk) + key). e0/e1: index of key j0 in rows r0 and r0 + 8.
+// Lane qd of a quad draws the Philox groups 2qd and 2qd + 1 (keys 16 qd .. 16 qd + 15) of both rows; the quad then
+// exchanges them, since every lane holds two keys of each of the eight groups.
+__device__ __forceinline__ uint32_t fl_keep_bits(uint64_t seed, uint64_t offset, uint64_t e0, uint64_t e1,
+                                                 uint32_t thr) {
+  const int lane = (int)lane_id(), qd = lane & 3;
+  uint32_t mine = 0;  // byte 2 ri + cc = the eight keep bits of group 2 qd + cc, row ri
+#pragma unroll
+  for (int ri = 0; ri < 2; ++ri)
+#pragma unroll
+    for (int cc = 0; cc < 2; ++cc) {
+      const Philox4 r = philox4x32(seed, offset, ((ri ? e1 : e0) + 16 * qd + 8 * cc) >> 3);
+#pragma unroll
+      for (int l = 0; l < 8; ++l)
+        if (philox_lane16(r, l) >= thr) mine |= 1u << (8 * (2 * ri + cc) + l);
+    }
+  uint32_t keep = 0;
+#pragma unroll
+  for (int src = 0; src < 4; ++src) {
+    const uint32_t x = __shfl_sync(0xffffffffu, mine, (lane & ~3) | src);
+#pragma unroll
+    for (int cc = 0; cc < 2; ++cc)
+#pragma unroll
+      for (int ri = 0; ri < 2; ++ri) {
+        const uint32_t bits = (x >> (8 * (2 * ri + cc) + 2 * qd)) & 3u;  // keys 2 qd, 2 qd + 1 of group 2 src + cc
+        keep |= bits << (4 * (2 * src + cc) + 2 * ri);
+      }
+  }
+  return keep;
+}
 
 template <bool RPE>
 __global__ void __launch_bounds__(FL_THREADS, 1)
     attn_flash_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                           const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_pe,
                           const FlashFwdParams p) {
+  constexpr int ST = fl_stages<RPE>();
+  constexpr uint32_t SB = fl_stage_bytes<RPE>();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                     // [64 rows][128 B]
-  uint8_t* sK = sQ + 8192;                // 2 x [64 keys][128 B]  (K-major B operand of S)
-  uint8_t* sV = sK + 2 * 8192;            // [64 keys][128 B]      (MN-major B operand of O)
-  uint8_t* sP = sV + 8192;                // [64 rows][64 keys]    (K-major A operand of O)
-  float* sS = reinterpret_cast<float*>(sP + 8192);  // [64][FL_SP] scores of the current step
-  float* sO = sS + FL_T * FL_SP;                    // [64][FL_SP] finished output accumulator
-  uint8_t* sPE = reinterpret_cast<uint8_t*>(sO + FL_T * FL_SP);  // RPE: 2 x [128 table rows][128 B]
-  float* sQP = reinterpret_cast<float*>(sPE + (RPE ? 2 * 16384 : 0));  // RPE: [64][FL_QPP]
-  uint64_t* bar_q = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sQP) + (RPE ? FL_T * FL_QPP * 4 : 0));
-  uint64_t* bar_k = bar_q + 1;        // [2] K (+ PEw) of a step landed
-  uint64_t* bar_kfree = bar_q + 3;    // [2] the score MMAs that read this K stage have completed
-  uint64_t* bar_s = bar_q + 5;        // scores of a step are in sS (+ sQP)
-  uint64_t* bar_sfree = bar_q + 6;    // softmax warps have read the scores of a step
-  uint64_t* bar_v = bar_q + 7;        // V block landed
-  uint64_t* bar_p = bar_q + 8;        // P tile written
-  uint64_t* bar_pv = bar_q + 9;       // P V MMAs of a block complete (sP and sV may be rewritten)
-  uint64_t* bar_o = bar_q + 10;       // O is in sO
-  float* red = reinterpret_cast<float*>(bar_q + 16);  // [2][64] row partials of the two column halves
+  uint8_t* sQ = smem;             // 2 x [64 rows][128 B], one tile per warpgroup
+  uint8_t* sStage = sQ + 2 * 8192;  // ST x { K [64 keys][128 B] (K-major B of S) | V [64 keys][128 B] (MN-major B of O)
+                                    //        | RPE: 2 x PEw [128 table rows][128 B] }
+  float* sQP = reinterpret_cast<float*>(sStage + ST * SB);  // RPE: 2 x [64][FL_QPP]
+  uint64_t* bar_q = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sQP) + (RPE ? 2 * FL_T * FL_QPP * 4 : 0));
+  uint64_t* bar_full = bar_q + 1;       // [ST] K (+ V in sweep 1, + PEw) of a stage landed
+  uint64_t* bar_free = bar_full + ST;   // [ST] every warpgroup's MMAs that read the stage have completed
 
   const int warp = threadIdx.x >> 5;
   const int nqt = (p.Tq + FL_T - 1) / FL_T;
-  const int qt = nqt - 1 - (int)blockIdx.x;  // late (long, when causal) tiles first
+  int ta, tb;
+  fl_tiles((int)blockIdx.x, nqt, p.causal != 0, ta, tb);
+  const int nwg = tb >= 0 ? 2 : 1;
   const int h = blockIdx.y, b = blockIdx.z;
-  const int i0 = qt * FL_T;
-  int tk = p.Tk;
-  if (p.causal && i0 + FL_T < tk) tk = i0 + FL_T;
-  const int nkb = (tk + FL_T - 1) / FL_T;
+  const int nkbm = fl_tile_nkb(ta, p.Tk, p.causal != 0);  // key blocks the longer tile needs
   void* const probs = (p.probs_heads > 0 && h >= p.probs_heads) ? nullptr : p.probs;  // (uniform over the CTA)
   const int nsweep = probs != nullptr ? 3 : 2;
-  const int NS = nsweep * nkb;
 
-  if (warp == 4 && elect_one()) {
+  if (warp == 8 && elect_one()) {
     tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_k);
     tma_prefetch_desc(&map_v);
     if constexpr (RPE) tma_prefetch_desc(&map_pe);
     mbar_init(bar_q, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bar_k[s], 1);
-      mbar_init(&bar_kfree[s], 1);
+    for (int s = 0; s < ST; ++s) {
+      mbar_init(&bar_full[s], 1);
+      mbar_init(&bar_free[s], nwg);
     }
-    mbar_init(bar_s, 128);
-    mbar_init(bar_sfree, 4);
-    mbar_init(bar_v, 1);
-    mbar_init(bar_p, 4);
-    mbar_init(bar_pv, 1);
-    mbar_init(bar_o, 128);
     fence_mbar_init();
   }
   __syncthreads();
   pdl_sync();  // (prologue done: nothing above touched global memory)
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (elect_one()) {
-      mbar_expect_tx(bar_q, 8192);
-      tma_load_4d(sQ, &map_q, bar_q, 0, i0, h, b);
-      int pv = 0;
+      mbar_expect_tx(bar_q, 8192u * nwg);
+      tma_load_4d(sQ, &map_q, bar_q, 0, ta * FL_T, h, b);
+      if (tb >= 0) tma_load_4d(sQ + 8192, &map_q, bar_q, 0, tb * FL_T, h, b);
+      const int NS = nsweep * nkbm;
       for (int s = 0; s < NS; ++s) {
-        const int sweep = s / nkb, kb = s - sweep * nkb;
-        const int st = s & 1;
-        if (s >= 2) mbar_wait_quiet(&bar_kfree[st], (uint32_t)(((s >> 1) - 1) & 1));
-        mbar_expect_tx(&bar_k[st], 8192u + (RPE ? 16384u : 0u));
-        tma_load_4d(sK + st * 8192, &map_k, &bar_k[st], 0, kb * FL_T, h, b);
-        if constexpr (RPE)
-          tma_load_4d(sPE + st * 16384, &map_pe, &bar_k[st], 0, fl_window_row0(i0, kb * FL_T, p.maxpos), 0, 0);
-        if (sweep == 1) {
-          if (pv > 0) mbar_wait_quiet(bar_pv, (uint32_t)((pv - 1) & 1));  // P V of the previous block has read sV
-          mbar_expect_tx(bar_v, 8192);
-          tma_load_4d(sV, &map_v, bar_v, 0, kb * FL_T, h, b);
-          ++pv;
+        const int sweep = s / nkbm, kb = s - sweep * nkbm, st = s % ST;
+        if (s >= ST) mbar_wait_quiet(&bar_free[st], (uint32_t)((s / ST - 1) & 1));
+        uint8_t* stg = sStage + st * SB;
+        mbar_expect_tx(&bar_full[st], (sweep == 1 ? 16384u : 8192u) + (RPE ? 16384u * nwg : 0u));
+        tma_load_4d(stg, &map_k, &bar_full[st], 0, kb * FL_T, h, b);
+        if (sweep == 1) tma_load_4d(stg + 8192, &map_v, &bar_full[st], 0, kb * FL_T, h, b);
+        if constexpr (RPE) {
+          tma_load_4d(stg + 16384, &map_pe, &bar_full[st], 0, fl_window_row0(ta * FL_T, kb * FL_T, p.maxpos), 0, 0);
+          if (tb >= 0)
+            tma_load_4d(stg + 32768, &map_pe, &bar_full[st], 0, fl_window_row0(tb * FL_T, kb * FL_T, p.maxpos), 0, 0);
         }
       }
     }
-  } else if (warp < 4) {
-    // ===================== MMA warpgroup =====================
-    mbar_wait_quiet(bar_q, 0);
-    const uint32_t aq = smem_u32(sQ), ap = smem_u32(sP), av = smem_u32(sV);
-    float o[32];
+    return;
+  }
+
+  // ===================== MMA warpgroups: thread = rows r0, r0 + 8 x 16 keys of every block =====================
+  const int wg = warp >> 2, wl = warp & 3;
+  const int t = wg == 0 ? ta : tb;
+  if (t < 0) return;  // second warpgroup of a lone tile
+  const bool lead = (threadIdx.x & 127) == 0;
+  const int i0 = t * FL_T;
+  int tk = p.Tk;
+  if (p.causal && i0 + FL_T < tk) tk = i0 + FL_T;
+  const int nkb = (tk + FL_T - 1) / FL_T;
+  const int lane = (int)lane_id(), qd = lane & 3;
+  const int r0 = 16 * wl + (lane >> 2);                      // local rows r0 and r0 + 8
+  const bool row_ok[2] = {i0 + r0 < p.Tq, i0 + r0 + 8 < p.Tq};
+  const int64_t prow0 = ((int64_t)b * p.H + h) * p.Tq + i0 + r0;  // row r0 + 8 ri: prow0 + 8 ri
+  const int rh = i0 + 32 * (wl >> 1);  // first row of this warp's 32-row half (the psave zero-fill granularity)
+  const uint8_t* kp = p.key_pad != nullptr ? p.key_pad + (int64_t)b * p.Tk : nullptr;
+  uint64_t dseed = p.seed, doffset = p.offset;
+  if (p.drop_thr != 0) resolve_seed(dseed, doffset);
+  const uint64_t dpitch = attn_drop_pitch(p.Tk);
+  float* probs_f = reinterpret_cast<float*>(probs);
+  __nv_bfloat16* probs_h = reinterpret_cast<__nv_bfloat16*>(probs);
+  const uint32_t aq = smem_u32(sQ + wg * 8192);
+  float* qpw = sQP + wg * FL_T * FL_QPP;
+
+  float o[32];
 #pragma unroll
-    for (int t = 0; t < 32; ++t) o[t] = 0.f;
-    int pv = 0;
-    for (int s = 0; s < NS; ++s) {
-      const int sweep = s / nkb;
-      const int st = s & 1;
-      mbar_wait_quiet(&bar_k[st], (uint32_t)((s >> 1) & 1));
-      if (s > 0) mbar_wait_quiet(bar_sfree, (uint32_t)((s - 1) & 1));
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, mm[2] = {0.f, 0.f}, sum[2] = {0.f, 0.f}, inv[2] = {0.f, 0.f};
+  mbar_wait_quiet(bar_q, 0);
+  for (int sweep = 0; sweep < nsweep; ++sweep) {
+    for (int kb = 0; kb < nkbm; ++kb) {
+      const int s = sweep * nkbm + kb, st = s % ST;
+      mbar_wait_quiet(&bar_full[st], (uint32_t)((s / ST) & 1));
+      if (kb >= nkb) {  // a block only the other (longer, causal) tile needs
+        if (lead) mbar_arrive(&bar_free[st]);
+        continue;
+      }
+      const int j0 = kb * FL_T;
+      const uint32_t astg = smem_u32(sStage + st * SB);
+      // which of this thread's elements count: key exists and is not padded (a byte per lane + ballot), causal, and
+      // the element's 32 x 32 chunk (rows of this warp's half, 32 keys) is live
+      uint32_t vm = 0;
+      bool live[2];
       {
-        float sc[32];
-        const uint32_t ak = smem_u32(sK + st * 8192);
+        const int ja = j0 + lane, jb = j0 + 32 + lane;
+        const uint32_t oka = __ballot_sync(0xffffffffu, ja < p.Tk && !(kp != nullptr && kp[ja] != 0));
+        const uint32_t okb = __ballot_sync(0xffffffffu, jb < p.Tk && !(kp != nullptr && kp[jb] != 0));
+#pragma unroll
+        for (int ch = 0; ch < 2; ++ch) {
+          const int jc = j0 + 32 * ch;
+          live[ch] = rh < p.Tq && jc < tk && !(p.causal && jc > rh + 31);
+        }
+        const uint64_t okk = (live[0] ? (uint64_t)oka : 0ull) | (live[1] ? (uint64_t)okb << 32 : 0ull);
+#pragma unroll
+        for (int ri = 0; ri < 2; ++ri) {
+          uint64_t rm = okk;  // bit j: key j0 + j counts for row r0 + 8 ri
+          if (p.causal) {
+            const int lim = i0 + r0 + 8 * ri - j0;  // keys j0 .. j0 + lim are visible
+            rm &= lim >= 63 ? ~0ull : (lim < 0 ? 0ull : (2ull << lim) - 1ull);
+          }
+          const uint32_t lo = (uint32_t)(rm >> (2 * qd)), hi = (uint32_t)(rm >> (32 + 2 * qd));
+#pragma unroll
+          for (int c = 0; c < 8; ++c)
+            vm |= (((c < 4 ? lo : hi) >> (8 * (c & 3))) & 3u) << (4 * c + 2 * ri);
+        }
+      }
+      // dropout keep bits (sweep 1), drawn before the MMAs so that no score fragment is live meanwhile
+      uint32_t keep = 0xffffffffu;
+      if (sweep == 1 && p.drop_thr != 0)
+        keep = fl_keep_bits(dseed, doffset, (uint64_t)prow0 * dpitch + j0, (uint64_t)(prow0 + 8) * dpitch + j0,
+                            p.drop_thr);
+      if constexpr (RPE) {  // QPw first, so that its fragment and the score fragment are never live together
+        float qp[64];
+        const uint32_t ape = astg + 16384 + wg * 16384;
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k)  // head dim 64 = 4 x 16
-          wgmma_m64n64<0, 0>(sc, wgmma_smem_desc(aq + k * 32, 16, 1024), wgmma_smem_desc(ak + k * 32, 16, 1024),
-                             k != 0 ? 1u : 0u);
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n128<0, 0>(qp, wgmma_smem_desc(aq + k * 32, 16, 1024), wgmma_smem_desc(ape + k * 32, 16, 1024),
+                              k != 0 ? 1u : 0u);
         wgmma_commit();
-        if constexpr (RPE) {
-          float qp[64];
-          const uint32_t ape = smem_u32(sPE + st * 16384);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            wgmma_m64n128<0, 0>(qp, wgmma_smem_desc(aq + k * 32, 16, 1024), wgmma_smem_desc(ape + k * 32, 16, 1024),
-                                k != 0 ? 1u : 0u);
-          wgmma_commit();
-          wgmma_wait<0>();
-          wgmma_fence_regs(qp);
-          fl_store_acc(sQP, FL_QPP, qp);
-        } else {
-          wgmma_wait<0>();
-        }
-        wgmma_fence_regs(sc);
-        if (threadIdx.x == 0) mbar_arrive(&bar_kfree[st]);
-        fl_store_acc(sS, FL_SP, sc);
+        wgmma_wait<0>();
+        wgmma_fence_regs(qp);
+        fl_bar_wg(1 + wg);  // every lane has read the previous block's window
+        fl_store_acc(qpw, FL_QPP, qp);
       }
-      mbar_arrive(bar_s);
-      if (sweep == 1) {
-        mbar_wait_quiet(bar_v, (uint32_t)(pv & 1));
-        mbar_wait_quiet(bar_p, (uint32_t)(pv & 1));
+      float sc[32];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)  // head dim 64 = 4 x 16
+        wgmma_m64n64<0, 0>(sc, wgmma_smem_desc(aq + k * 32, 16, 1024), wgmma_smem_desc(astg + k * 32, 16, 1024),
+                           k != 0 ? 1u : 0u);
+      wgmma_commit();
+      if constexpr (RPE) fl_bar_wg(1 + wg);  // the window is complete (while the score MMAs run)
+      wgmma_wait<0>();
+      wgmma_fence_regs(sc);
+      if (sweep != 1 && lead) mbar_arrive(&bar_free[st]);
+      if constexpr (RPE) {
+        // row i, key j  ->  window column i - j + maxpos - w0, clamped to [0, colmax] (the table ends)
+        const int w0 = fl_window_row0(i0, j0, p.maxpos);
+        int colmax = 2 * p.maxpos - 1 - w0;
+        if (colmax > FL_PE_ROWS - 1) colmax = FL_PE_ROWS - 1;
+        const int off = i0 + r0 - j0 - 2 * qd + p.maxpos - w0;  // column of row r0, key j0 + 2 qd
+        const float* qrow = qpw + r0 * FL_QPP;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int ri = (i >> 1) & 1;
+          int col = off + 8 * ri - 8 * (i >> 2) - (i & 1);
+          col = col < 0 ? 0 : (col > colmax ? colmax : col);
+          sc[i] += qrow[8 * ri * FL_QPP + col];
+        }
+      }
+      if (sweep == 0) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+          if ((vm >> i) & 1u) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], sc[i] * p.scale_log2);
+      } else if (sweep == 1) {
+        uint32_t pa[4][4];  // P as the A operand of P V: 16 keys per four registers
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+          const int ri = (i >> 1) & 1, c = i >> 2;
+          const float e0 = ((vm >> i) & 1u) ? fast_ex2(sc[i] * p.scale_log2 - mm[ri]) : 0.f;
+          const float e1 = ((vm >> (i + 1)) & 1u) ? fast_ex2(sc[i + 1] * p.scale_log2 - mm[ri]) : 0.f;
+          sum[ri] += e0;
+          sum[ri] += e1;
+          const bool k0 = (keep >> i) & 1u, k1 = (keep >> (i + 1)) & 1u;
+          pa[c >> 1][(c & 1) << 1 | ri] =
+              fl_pack(k0 ? e0 * p.drop_scale : 0.f, k1 ? e1 * p.drop_scale : 0.f);
+          const int jcol = j0 + 8 * c;
+          if (p.psave != nullptr && row_ok[ri] && jcol + 8 <= p.p_ld)
+            *reinterpret_cast<uint32_t*>(p.psave + (prow0 + 8 * ri) * p.p_ld + jcol + 2 * qd) =
+                live[c >> 2] ? fl_pack(k0 ? e0 : -e0, k1 ? e1 : -e1) : 0u;
+        }
+        const uint32_t av = astg + 8192;
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k)  // 64 keys = 4 x 16
-          wgmma_m64n64<0, 1>(o, wgmma_smem_desc(ap + k * 32, 16, 1024), wgmma_smem_desc(av + k * 2048, 8192, 1024),
-                             (pv | k) != 0 ? 1u : 0u);
+          wgmma_m64n64_rs<1>(o, pa[k], wgmma_smem_desc(av + k * 2048, 8192, 1024), 1u);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(o);
-        if (threadIdx.x == 0) mbar_arrive(bar_pv);
-        ++pv;
-      }
-    }
-    fl_store_acc(sO, FL_SP, o);
-    mbar_arrive(bar_o);
-  } else {
-    // ===================== softmax warps: thread = (query row, 32-key chunk `half` of every block) =====================
-    const int sw = warp - 5;
-    const int q = sw & 1;                   // rows [32 q, 32 q + 32) of the tile
-    const int half = sw >> 1;               // 0 / 1
-    const int lane = (int)lane_id();
-    const int r = q * 32 + lane;
-    const int i = i0 + r;
-    const bool row_ok = i < p.Tq;
-    const bool warp_live = i0 + q * 32 < p.Tq;
-    const uint8_t* kp = p.key_pad != nullptr ? p.key_pad + (int64_t)b * p.Tk : nullptr;
-    const int64_t prow = ((int64_t)b * p.H + h) * p.Tq + i;
-    uint64_t dseed = p.seed, doffset = p.offset;
-    if (p.drop_thr != 0) resolve_seed(dseed, doffset);
-    float* probs_f = reinterpret_cast<float*>(probs);
-    __nv_bfloat16* probs_h = reinterpret_cast<__nv_bfloat16*>(probs);
-
-    float m = -INFINITY, mm = 0.f, sum = 0.f, inv = 0.f;
-    int pv = 0;
-    for (int sweep = 0; sweep < nsweep; ++sweep) {
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = sweep * nkb + kb;
-        const int j0 = kb * FL_T;
-        mbar_wait_quiet(bar_s, (uint32_t)(s & 1));
-        if (sweep == 1 && pv > 0) mbar_wait_quiet(bar_pv, (uint32_t)((pv - 1) & 1));  // sP is free again
-        const int c = half;  // 32-key chunk of the block
-        const int jc = j0 + c * 32;
-        // warp-uniform: does any (row, key) pair of this 32 x 32 chunk exist and pass the causal mask?
-        const bool live = warp_live && jc < tk && !(p.causal && jc > i0 + q * 32 + 31);
-        uint8_t* blk = sP + r * 128;
-        const int cbase = c * 4;
-        if (!live) {
-          if (sweep == 1) {  // the P V MMA contracts over these keys and the backward reads psave: zeros
+        fl_fence_u32(pa);
+        if (lead) mbar_arrive(&bar_free[st]);  // K and V of the stage are both read
+      } else {  // sweep 2: normalised, undropped probabilities for the caller
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              *reinterpret_cast<uint4*>(blk + (((cbase + g) ^ (r & 7)) << 4)) = make_uint4(0u, 0u, 0u, 0u);
-              if (p.psave != nullptr && row_ok && jc + 8 * g + 8 <= p.p_ld)
-                *reinterpret_cast<uint4*>(p.psave + prow * p.p_ld + jc + 8 * g) = make_uint4(0u, 0u, 0u, 0u);
-            }
-          } else if (sweep == 2 && row_ok) {
-            for (int t = 0; t < 32; ++t)
-              if (jc + t < p.p_ld) {
-                if (p.probs_fp32) probs_f[prow * p.p_ld + jc + t] = 0.f;
-                else probs_h[prow * p.p_ld + jc + t] = __float2bfloat16(0.f);
-              }
+        for (int i = 0; i < 32; ++i) {
+          const int ri = (i >> 1) & 1;
+          const int j = j0 + 8 * (i >> 2) + 2 * qd + (i & 1);
+          if (row_ok[ri] && j < p.p_ld) {
+            const float pr = ((vm >> i) & 1u) ? fast_ex2(sc[i] * p.scale_log2 - mm[ri]) * inv[ri] : 0.f;
+            if (p.probs_fp32) probs_f[(prow0 + 8 * ri) * p.p_ld + j] = pr;
+            else probs_h[(prow0 + 8 * ri) * p.p_ld + j] = __float2bfloat16(pr);
           }
-        } else {
-          float v[32];
-          {
-            const float* src = sS + r * FL_SP + c * 32;
-#pragma unroll
-            for (int t = 0; t < 32; t += 4) {
-              const float4 f = *reinterpret_cast<const float4*>(src + t);
-              v[t] = f.x; v[t + 1] = f.y; v[t + 2] = f.z; v[t + 3] = f.w;
-            }
-          }
-          // validity bits of this row's 32 keys: key exists, not padded (one byte load per lane + ballot), causal
-          uint32_t vb;
-          {
-            const int j = jc + lane;
-            const bool ok = j < tk && !(kp != nullptr && kp[j] != 0);
-            vb = __ballot_sync(0xffffffffu, ok);
-            if (p.causal) {
-              const int lim = i - jc;  // keys 0..lim of the chunk are visible
-              vb &= lim >= 31 ? 0xffffffffu : (lim < 0 ? 0u : ((2u << lim) - 1u));
-            }
-          }
-          if constexpr (RPE) {
-            // row i, key j = jc + u  ->  window column i - j + maxpos - w0, clamped to [0, colmax] (the table ends)
-            const int w0 = fl_window_row0(i0, j0, p.maxpos);
-            int colmax = 2 * p.maxpos - 1 - w0;
-            if (colmax > FL_PE_ROWS - 1) colmax = FL_PE_ROWS - 1;
-            const int off = i - jc + p.maxpos - w0;
-            const float* qrow = sQP + r * FL_QPP;
-#pragma unroll
-            for (int t = 0; t < 32; ++t) {
-              int col = off - t;
-              col = col < 0 ? 0 : (col > colmax ? colmax : col);
-              v[t] += qrow[col];
-            }
-          }
-          if (sweep == 0) {
-#pragma unroll
-            for (int t = 0; t < 32; ++t)
-              if ((vb >> t) & 1u) m = fmaxf(m, v[t] * p.scale_log2);
-          } else if (sweep == 1) {
-            uint32_t kb_ = 0xffffffffu;
-            if (p.drop_thr != 0)
-              kb_ = dropout_keep_mask32(dseed, doffset, (uint64_t)prow * attn_drop_pitch(p.Tk) + (uint64_t)jc, p.drop_thr);
-            __nv_bfloat16* psv = (p.psave != nullptr && row_ok) ? p.psave + prow * p.p_ld + jc : nullptr;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              float ev[8];
-#pragma unroll
-              for (int t = 0; t < 8; ++t) {
-                const int u = 8 * g + t;
-                ev[t] = ((vb >> u) & 1u) ? fast_ex2(v[u] * p.scale_log2 - mm) : 0.f;
-                sum += ev[t];
-              }
-              const uint32_t k8 = kb_ >> (8 * g);
-              uint4 pk, ps;
-              pk.x = fl_pack((k8 & 1u) ? ev[0] * p.drop_scale : 0.f, (k8 & 2u) ? ev[1] * p.drop_scale : 0.f);
-              pk.y = fl_pack((k8 & 4u) ? ev[2] * p.drop_scale : 0.f, (k8 & 8u) ? ev[3] * p.drop_scale : 0.f);
-              pk.z = fl_pack((k8 & 16u) ? ev[4] * p.drop_scale : 0.f, (k8 & 32u) ? ev[5] * p.drop_scale : 0.f);
-              pk.w = fl_pack((k8 & 64u) ? ev[6] * p.drop_scale : 0.f, (k8 & 128u) ? ev[7] * p.drop_scale : 0.f);
-              *reinterpret_cast<uint4*>(blk + (((cbase + g) ^ (r & 7)) << 4)) = pk;
-              if (psv != nullptr && jc + 8 * g + 8 <= p.p_ld) {
-                ps.x = fl_pack((k8 & 1u) ? ev[0] : -ev[0], (k8 & 2u) ? ev[1] : -ev[1]);
-                ps.y = fl_pack((k8 & 4u) ? ev[2] : -ev[2], (k8 & 8u) ? ev[3] : -ev[3]);
-                ps.z = fl_pack((k8 & 16u) ? ev[4] : -ev[4], (k8 & 32u) ? ev[5] : -ev[5]);
-                ps.w = fl_pack((k8 & 64u) ? ev[6] : -ev[6], (k8 & 128u) ? ev[7] : -ev[7]);
-                *reinterpret_cast<uint4*>(psv + 8 * g) = ps;
-              }
-            }
-          } else if (row_ok) {  // sweep 2: normalised, undropped probabilities for the caller
-            if (p.probs_fp32) {
-              float* dst = probs_f + prow * p.p_ld + jc;
-              if (jc + 32 <= p.p_ld && (p.p_ld & 3) == 0) {
-#pragma unroll
-                for (int t = 0; t < 32; t += 4) {
-                  float4 o4;
-                  o4.x = ((vb >> t) & 1u) ? fast_ex2(v[t] * p.scale_log2 - mm) * inv : 0.f;
-                  o4.y = ((vb >> (t + 1)) & 1u) ? fast_ex2(v[t + 1] * p.scale_log2 - mm) * inv : 0.f;
-                  o4.z = ((vb >> (t + 2)) & 1u) ? fast_ex2(v[t + 2] * p.scale_log2 - mm) * inv : 0.f;
-                  o4.w = ((vb >> (t + 3)) & 1u) ? fast_ex2(v[t + 3] * p.scale_log2 - mm) * inv : 0.f;
-                  *reinterpret_cast<float4*>(dst + t) = o4;
-                }
-              } else {
-#pragma unroll
-                for (int t = 0; t < 32; ++t)
-                  if (jc + t < p.p_ld) dst[t] = ((vb >> t) & 1u) ? fast_ex2(v[t] * p.scale_log2 - mm) * inv : 0.f;
-              }
-            } else {
-              __nv_bfloat16* dst = probs_h + prow * p.p_ld + jc;
-#pragma unroll
-              for (int t = 0; t < 32; ++t)
-                if (jc + t < p.p_ld)
-                  dst[t] = __float2bfloat16(((vb >> t) & 1u) ? fast_ex2(v[t] * p.scale_log2 - mm) * inv : 0.f);
-            }
-          }
-        }
-        if (sweep == 1) {
-          fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_p);
-          ++pv;
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_sfree);
-      }
-      if (sweep == 0) {  // the row maximum over all keys: combine the two column halves
-        red[half * FL_T + r] = m;
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        m = fmaxf(red[r], red[FL_T + r]);
-        mm = m == -INFINITY ? 0.f : m;
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-      } else if (sweep == 1) {
-        red[half * FL_T + r] = sum;
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        sum = red[r] + red[FL_T + r];
-        inv = sum > 0.f ? 1.f / sum : 0.f;
-        if (half == 0 && row_ok) {
-          if (p.lse != nullptr) p.lse[prow] = sum > 0.f ? (mm + log2f(sum)) * 0.6931471805599453f : -INFINITY;
-          if (p.inv_l != nullptr) p.inv_l[prow] = inv;
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-      } else if (p.causal && half == 0 && row_ok) {  // probabilities right of the last visible block
-        for (int j = nkb * FL_T; j < (int)p.p_ld; ++j) {
-          if (p.probs_fp32) probs_f[prow * p.p_ld + j] = 0.f;
-          else probs_h[prow * p.p_ld + j] = __float2bfloat16(0.f);
         }
       }
     }
-    // ---- epilogue: O / rowsum; this thread owns channels [32 half, 32 half + 32) of its row
-    mbar_wait_quiet(bar_o, 0);
-    if (row_ok) {
-      float v[32];
-      const float* src = sO + r * FL_SP + half * 32;
+    // end of a sweep: combine each row over its quad
+    if (sweep == 0) {
 #pragma unroll
-      for (int t = 0; t < 32; t += 4) {
-        const float4 f = *reinterpret_cast<const float4*>(src + t);
-        v[t] = f.x * inv; v[t + 1] = f.y * inv; v[t + 2] = f.z * inv; v[t + 3] = f.w * inv;
+      for (int ri = 0; ri < 2; ++ri) {
+        m[ri] = fmaxf(m[ri], __shfl_xor_sync(0xffffffffu, m[ri], 1));
+        m[ri] = fmaxf(m[ri], __shfl_xor_sync(0xffffffffu, m[ri], 2));
+        mm[ri] = m[ri] == -INFINITY ? 0.f : m[ri];
       }
-      if (p.out_f32 != nullptr) {
-        float* d32 = p.out_f32 + ((int64_t)b * p.Tq + i) * (p.H * 64) + h * 64 + half * 32;
+    } else if (sweep == 1) {
 #pragma unroll
-        for (int t = 0; t < 32; t += 4) *reinterpret_cast<float4*>(d32 + t) = make_float4(v[t], v[t + 1], v[t + 2], v[t + 3]);
+      for (int ri = 0; ri < 2; ++ri) {
+        sum[ri] += __shfl_xor_sync(0xffffffffu, sum[ri], 1);
+        sum[ri] += __shfl_xor_sync(0xffffffffu, sum[ri], 2);
+        inv[ri] = sum[ri] > 0.f ? 1.f / sum[ri] : 0.f;
+        if (qd == 0 && row_ok[ri]) {
+          const int64_t pr = prow0 + 8 * ri;
+          if (p.lse != nullptr) p.lse[pr] = sum[ri] > 0.f ? (mm[ri] + log2f(sum[ri])) * 0.6931471805599453f : -INFINITY;
+          if (p.inv_l != nullptr) p.inv_l[pr] = inv[ri];
+        }
       }
-      __nv_bfloat16* dst = p.out + (int64_t)b * p.o_bs + (int64_t)i * p.o_ld + h * 64 + half * 32;
+    } else if (p.causal) {  // probabilities right of the last visible block
 #pragma unroll
-      for (int t = 0; t < 32; t += 8) {
-        uint4 pk;
-        pk.x = fl_pack(v[t], v[t + 1]);
-        pk.y = fl_pack(v[t + 2], v[t + 3]);
-        pk.z = fl_pack(v[t + 4], v[t + 5]);
-        pk.w = fl_pack(v[t + 6], v[t + 7]);
-        *reinterpret_cast<uint4*>(dst + t) = pk;
-      }
+      for (int ri = 0; ri < 2; ++ri)
+        if (row_ok[ri])
+          for (int j = nkb * FL_T + qd; j < (int)p.p_ld; j += 4) {
+            if (p.probs_fp32) probs_f[(prow0 + 8 * ri) * p.p_ld + j] = 0.f;
+            else probs_h[(prow0 + 8 * ri) * p.p_ld + j] = __float2bfloat16(0.f);
+          }
+    }
+  }
+  // ---- epilogue: O / rowsum straight from the fragments
+#pragma unroll
+  for (int ri = 0; ri < 2; ++ri) {
+    if (!row_ok[ri]) continue;
+    const int i = i0 + r0 + 8 * ri;
+    float* d32 = p.out_f32 != nullptr ? p.out_f32 + ((int64_t)b * p.Tq + i) * (p.H * 64) + h * 64 + 2 * qd : nullptr;
+    __nv_bfloat16* dst = p.out + (int64_t)b * p.o_bs + (int64_t)i * p.o_ld + h * 64 + 2 * qd;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      const float v0 = o[4 * c + 2 * ri] * inv[ri], v1 = o[4 * c + 2 * ri + 1] * inv[ri];
+      if (d32 != nullptr) *reinterpret_cast<float2*>(d32 + 8 * c) = make_float2(v0, v1);
+      *reinterpret_cast<uint32_t*>(dst + 8 * c) = fl_pack(v0, v1);
     }
   }
 }
@@ -467,7 +454,7 @@ static int fl_launch(const st5_attn_args* a, float* lse, void* psave, float* inv
   p.drop_thr = drop_threshold(a->drop_p);
   p.drop_scale = a->drop_p > 0.f ? 1.f / (1.f - a->drop_p) : 1.f;
   p.seed = a->seed; p.offset = a->offset;
-  dim3 grid((a->Tq + FL_T - 1) / FL_T, a->H, a->B);
+  dim3 grid(((a->Tq + FL_T - 1) / FL_T + 1) / 2, a->H, a->B);  // two query tiles per CTA
   if (rpe)
     launch_pdl(attn_flash_fwd_kernel<true>, grid, dim3(FL_THREADS), fl_smem<true>(), (cudaStream_t)stream, mq, mk, mv, mpe, p);
   else
