@@ -1,7 +1,9 @@
 """-m gpu: st5_gemm_bf16 (csrc/gemm.cu) against its contract in include/speecht5_b200.h, stated in fp64 by
 tests/gemm_emulator.gemm on CPU copies of the same operands, with ELEMENTWISE bounds (one wrong 32 x 32 block, a dropped
 k-block or one wrong mask bit fails), NaN sentinels around every output and in every operand's padding, and dropout
-masks compared bit for bit with tests/dropout_ref.py.
+masks compared bit for bit with tests/dropout_ref.py. The test_core_window_* cases hand the kernel the overlapping
+window operands of the convolutions (ld < K, or ld < rows MN-major), with NaN right after the last element a window
+reads.
 
 The tile width (128 x 64 or 128 x 128) is chosen by a cost model once per call and ST5_GEMM_BN pins it for a whole
 process, so the test_core_* cases run here with the cost model's choice and again in two child processes with each
@@ -60,6 +62,26 @@ class Operand:
         return {f"{which}_mn": self.mn, f"{which}_ld": self.ld, f"{which}_bs": (self.bs1, self.bs2)}
 
 
+class WindowOperand(Operand):
+    """bf16 operand rows x K read as an overlapping window, the layout of the convolutions: K-major with ld < K (row r
+    is the K elements from r * ld) or MN-major with ld < rows (k-row k is the rows elements from k * ld). The memory
+    past the logical K of a row (past `rows` of a k-row) is valid data of the next rows, finite; the zero fill of the
+    TMA map (dims[0] = K, or rows) alone keeps it out of a ragged last block. NaN starts right after the last element
+    a window may read, (rows - 1) ld + K (MN-major: (K - 1) ld + rows), and fills the gap between batch entries."""
+
+    def __init__(self, rows, K, mn, ld, nb1=1, gen=None, scale=1.0, dev="cuda"):
+        assert ld < (rows if mn else K), "not an overlapping window"
+        span = (K - 1) * ld + rows if mn else (rows - 1) * ld + K
+        self.ld, self.mn = ld, mn
+        self.bs1 = 0 if nb1 == 1 else _r8(span) + 16
+        self.bs2 = 0
+        buf = torch.full(((nb1 - 1) * self.bs1 + span + 64,), NAN, dtype=torch.float32)
+        for b1 in range(nb1):
+            buf[b1 * self.bs1:b1 * self.bs1 + span] = torch.randn(span, generator=gen) * scale
+        self.cpu = buf.to(torch.bfloat16)
+        self.dev = self.cpu.to(dev)
+
+
 class OutLayout:
     """Logical [nb2][nb1][M][N] region at pitch c_ld inside a larger buffer (rows past M, columns past N, gaps between
     batch entries and guard zones before and after); `inside` marks the logical elements."""
@@ -106,16 +128,19 @@ def _act_f64(v, act):
 def run_gemm(M, N, K, *, a_mn=False, b_mn=False, nb1=1, nb2=1, a_bcast=(False, False), b_bcast=(False, False),
              out_dtype=torch.float32, c_ld=None, shared=False, misalign=0, alpha=1.0, accumulate=0, bias=None,
              bias2_rows=0, residual=False, c_pre=False, act=None, actgrad_act=None, drop_p=0.0, seed=1234,
-             offset=7, device_seed=False, operand_scale=None, seed_data=0, check=True):
+             offset=7, device_seed=False, operand_scale=None, seed_data=0, check=True, a_win=None, b_win=None):
     """Run K.gemm on NaN-guarded buffers, then compare with the fp64 statement elementwise. Returns a dict of the CPU
-    results (got / ref regions, pre-activation, keep mask) for case-specific checks."""
+    results (got / ref regions, pre-activation, keep mask) for case-specific checks. a_win / b_win: the row pitch of
+    an overlapping-window operand (WindowOperand, nb2 = 1)."""
     from speecht5_b200 import kernels as K_
     dev = torch.device("cuda")
     gen = torch.Generator().manual_seed(seed_data)
     # operand scale: the pre-activation has unit standard deviation whatever K is
     sc = operand_scale if operand_scale is not None else K ** -0.25
-    A = Operand(M, K, a_mn, nb1, nb2, *a_bcast, gen=gen, scale=sc)
-    B = Operand(N, K, b_mn, nb1, nb2, *b_bcast, gen=gen, scale=sc)
+    A = WindowOperand(M, K, a_mn, a_win, nb1, gen=gen, scale=sc) if a_win else \
+        Operand(M, K, a_mn, nb1, nb2, *a_bcast, gen=gen, scale=sc)
+    B = WindowOperand(N, K, b_mn, b_win, nb1, gen=gen, scale=sc) if b_win else \
+        Operand(N, K, b_mn, nb1, nb2, *b_bcast, gen=gen, scale=sc)
     L = OutLayout(M, N, nb1, nb2, c_ld=c_ld, shared=shared, misalign=misalign)
     c0 = L.buffer(out_dtype, fill="randn" if accumulate == 1 else ("zero" if accumulate == 2 else None), gen=gen)
     if accumulate == 2 and shared:
@@ -248,6 +273,44 @@ def test_core_broadcast_b(cuda, major, out_dtype):
     """B shared by every batch entry (b_bs = 0): the layout of the relative-position contractions (Q PE^T, dQP PE)."""
     run_gemm(150, 320, 64, a_mn=major[0], b_mn=major[1], nb1=4, nb2=2, b_bcast=(True, True), out_dtype=out_dtype,
              seed_data=6)
+
+
+# Overlapping windows of the convolutions (rows, K, ld, nb1): row r of a K-major window is the K elements from r * ld.
+# Post-net Conv1d k5 (ld = C, K = 5 C), front-end layers 1-4 (ld = 2 C, K = 3 C), the positional conv (ld = cg = 48 / 64,
+# K = 128 cg: a row pitch of 96 / 128 bytes, not a multiple of the 128-byte swizzle span for 48), and each family again
+# with a ragged last k-block (K % 64 != 0).
+KWINDOWS = {"postnet80": (300, 400, 80, 2), "postnet256": (200, 1280, 256, 1), "postnet88_ragged": (130, 440, 88, 2),
+            "frontend512": (150, 1536, 1024, 2), "frontend200_ragged": (90, 600, 400, 2),
+            "posconv48": (130, 6144, 48, 1), "posconv64": (130, 8192, 64, 1), "posconv48_ragged": (70, 624, 48, 2),
+            "posconv64_ragged": (70, 8168, 64, 1)}
+# MN-major windows (rows, K, ld, nb1): k-row k is the `rows` elements from k * ld -- the B operand of the weight
+# gradients, ld = s C and rows = k C (strided layers, s = 2, k = 3) or ld = C and rows = 5 C (post-net).
+MWINDOWS = {"strided64_ragged": (192, 300, 128, 2), "strided512_ragged": (1536, 200, 1024, 1),
+            "postnet80": (400, 704, 80, 1), "postnet80_ragged": (400, 700, 80, 2)}
+SIDES = [("a", False), ("a", True), ("b", False), ("b", True)]
+SIDE_IDS = ["win_a-b_k", "win_a-b_mn", "win_b-a_k", "win_b-a_mn"]
+
+
+def _run_window(case, mn, side, other_mn, seed):
+    rows, K, ld, nb1 = case
+    if side == "a":
+        run_gemm(rows, 136, K, a_mn=mn, b_mn=other_mn, nb1=nb1, a_win=ld, seed_data=seed)
+    else:
+        run_gemm(136, rows, K, a_mn=other_mn, b_mn=mn, nb1=nb1, b_win=ld, seed_data=seed)
+
+
+@pytest.mark.parametrize("side", SIDES, ids=SIDE_IDS)
+@pytest.mark.parametrize("case", list(KWINDOWS), ids=list(KWINDOWS))
+def test_core_window_k_major(cuda, case, side):
+    """A K-major overlapping-window operand (ld < K) against either major of the other operand, on either side."""
+    _run_window(KWINDOWS[case], False, side[0], side[1], seed=31)
+
+
+@pytest.mark.parametrize("side", SIDES, ids=SIDE_IDS)
+@pytest.mark.parametrize("case", list(MWINDOWS), ids=list(MWINDOWS))
+def test_core_window_mn_major(cuda, case, side):
+    """An MN-major overlapping-window operand (ld < rows) against either major of the other operand, on either side."""
+    _run_window(MWINDOWS[case], True, side[0], side[1], seed=32)
 
 
 def test_core_cases_under_both_pinned_tile_widths(cuda):
