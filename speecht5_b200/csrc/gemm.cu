@@ -534,7 +534,17 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
+// cuTensorMapEncodeTiled is a driver-API call and needs a current context on the calling thread. The runtime binds its
+// primary context to a thread only at that thread's first runtime call, so on a thread whose first CUDA work is a GEMM
+// (autograd's device thread when a backward pass starts with a projection) the encode failed with
+// CUDA_ERROR_INVALID_CONTEXT. cudaSetDevice binds the primary context of the thread's current device (no synchronisation).
 static EncodeTiledFn get_encode_fn() {
+  static thread_local bool bound = false;
+  if (!bound) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess) cudaSetDevice(dev);
+    bound = true;
+  }
   static EncodeTiledFn fn = nullptr;
   static std::once_flag once;
   std::call_once(once, [] {
