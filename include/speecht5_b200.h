@@ -256,8 +256,8 @@ int st5_beam_topk(const void* logits, int64_t ld, int dtype, int32_t B, int32_t 
  * ignored) the hypothesis is appended while fin_n < K; the sentence is finished at fin_n == K or t == max_len.
  * Otherwise the first K non-eos candidates (then eos ones, which become ignored) continue: parent[r], cur_tok[r],
  * cur_score[r], lin[r][0..t] = lin[parent][0..t], lin[r][t+1] = r, tok / score[r][t+1]. stop[*t] = 1 when every
- * sentence is finished. t + 2 <= T is required (the caller sizes T). Returns -2 for K / T out of range, -3 for a NULL
- * pointer. */
+ * sentence is finished. t + 2 <= T is required (the caller sizes T). Returns -2 for K / T out of range or V <= K (step
+ * 0 has n = V - 1 < K candidates then, too few to continue K slots), -3 for a NULL pointer. */
 int st5_beam_update(int32_t B, int32_t K, int32_t V, int32_t T, int32_t eos, const int64_t* t, const int64_t* max_len,
                     int32_t normalize, float len_penalty, const float* cand_score, const int32_t* cand_token,
                     const int32_t* cand_beam, int32_t* lin, int32_t* tok, float* score, int32_t* ignore,

@@ -280,7 +280,8 @@ int beam_update_launch(int B, int K, int V, int T, int eos, const int64_t* t, co
                        int32_t* lin, int32_t* tok, float* score, int32_t* ignore, int32_t* finished, int32_t* parent,
                        int64_t* cur_tok, float* cur_score, int32_t* fin_n, int32_t* fin_tok, float* fin_pos,
                        int32_t* fin_len, float* fin_score, int32_t* stop, cudaStream_t st) {
-  if (B <= 0 || K < 1 || K > BKMAX || V < 2 || V > BVMAX || T < 2) return -2;
+  // (V > K: step 0 offers n = min(2K, V - 1) candidates, and K of them must continue)
+  if (B <= 0 || K < 1 || K > BKMAX || V <= K || V > BVMAX || T < 2) return -2;
   if (!t || !max_len || !cand_score || !cand_token || !cand_beam || !lin || !tok || !score || !ignore || !finished ||
       !parent || !cur_tok || !cur_score || !fin_n || !fin_tok || !fin_pos || !fin_len || !fin_score || !stop)
     return -3;

@@ -181,6 +181,7 @@ def test_argument_errors_are_reported_without_a_device():
     assert topk(2, 81, 81, p=None) == -3 and topk(2, 81, 80) == -6
     upd = lambda K, T, p=one: lib.st5_beam_update(1, K, 81, T, 2, p, p, 1, 1.0, *([p] * 17), None)  # noqa
     assert upd(17, 64) == -2 and upd(2, 1) == -2 and upd(2, 64, p=None) == -3
+    assert lib.st5_beam_update(1, 4, 4, 64, 2, one, one, 1, 1.0, *([one] * 17), None) == -2  # (V <= K)
     a = _lib.AttnLineageArgs()
     a.base.B, a.base.H, a.base.Tk, a.base.k, a.base.v, a.kv_div = 1, 1, 8, 16, 16, 0
     assert lib.st5_attn_lineage_fwd(C.byref(a), None) == -2

@@ -262,3 +262,23 @@ def test_full_size_base_beam5_graph(cuda):
         sc = [float(h["score"]) for h in gr]
         assert sc == sorted(sc, reverse=True) and all(math.isfinite(x) for x in sc)
         assert [h["tokens"].tolist() for h in e] == [h["tokens"].tolist() for h in gr]
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
+def test_hypotheses_past_130_tokens_graph_eager_and_batch1(cuda, dtype):
+    """min_len 132 of max_len 160 on the fixture model: the graph's buffers and position table well past the fixture's
+    16 steps (bucket 256). Graph and eager agree bit for bit; each sentence alone gives its row of the batch."""
+    blob = load()
+    m = _fixture_model(cuda, dtype, blob)
+    source, pm = torch.from_numpy(blob["in/source"]).to(cuda), torch.from_numpy(blob["in/padding_mask"]).to(cuda)
+    kw = dict(beam_size=4, max_len_b=160, min_len=132, **MASK_KW)
+    graph = m.generate_text_beam(source, pm, use_cache="graph", **kw)
+    eager = m.generate_text_beam(source, pm, use_cache=True, **kw)
+    for e, g in zip(eager, graph):
+        assert len(g) == 4 and all(len(h["tokens"]) > 130 for h in g)
+        assert [h["tokens"].tolist() for h in e] == [h["tokens"].tolist() for h in g]
+        assert [float(h["score"]) for h in e] == [float(h["score"]) for h in g]
+        assert all(torch.equal(a["positional_scores"], b["positional_scores"]) for a, b in zip(e, g))
+    for b in range(source.shape[0]):
+        one = m.generate_text_beam(source[b:b + 1], pm[b:b + 1], use_cache="graph", **kw)[0]
+        assert [h["tokens"].tolist() for h in one] == [h["tokens"].tolist() for h in graph[b]], b
