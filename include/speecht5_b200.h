@@ -245,6 +245,18 @@ int st5_beam_topk(const void* logits, int64_t ld, int dtype, int32_t B, int32_t 
                   const int64_t* max_len, float* cand_score, int32_t* cand_token, int32_t* cand_beam, float* ws,
                   void* stream);
 
+/* st5_beam_topk with a language model's log-probabilities fused in (sequence_generator.py:420-426, lm_weight w): per row,
+ * fp32, before any of st5_beam_topk's masking,
+ *   lp = (x / T - logsumexp(x / T)) + w * (y - logsumexp_{u < V_lm}(y_u))   for v < V_lm  (y = lm_logits[r * lm_ld + v],
+ *   ST5_F32 or ST5_BF16 per lm_dtype; no temperature on the LM), lp = x / T - logsumexp(x / T) for V_lm <= v < V;
+ * then eos -> -inf while *t < *min_len, NaN -> -inf (so w = 0 against an LM log-probability of -inf, or a NaN LM row,
+ * gives -inf), mask, max_len and cum exactly as st5_beam_topk, and the same selection into cand_*. Returns -2 for V_lm
+ * outside [1, V], -6 unless lm_ld >= V_lm, otherwise the codes of st5_beam_topk; nothing is launched on an error. */
+int st5_beam_topk_lm(const void* logits, int64_t ld, int dtype, int32_t B, int32_t K, int32_t V, const float* cum,
+                     const float* mask, float inv_temp, int32_t eos, const int64_t* t, const int64_t* min_len,
+                     const int64_t* max_len, float* cand_score, int32_t* cand_token, int32_t* cand_beam, float* ws,
+                     const void* lm_logits, int64_t lm_ld, int lm_dtype, int32_t V_lm, float lm_weight, void* stream);
+
 /* Beam search bookkeeping for step *t (sequence_generator.py:487-636 with finalize_hypos / is_finished :690-816), one
  * CTA per sentence; a sentence with finished[s] != 0 is skipped. State of slot r (= s * K + k), capacity T positions:
  *   lin[r][j]  the slot whose cells hold position j of the hypothesis now in slot r (lin[r][t] == r on entry);

@@ -88,6 +88,8 @@ _PROTOS = {
     "st5_beam_topk_ws_floats": (C.c_int64, [_i32, _i32]),
     "st5_beam_topk": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _f, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                 _vp]),
+    "st5_beam_topk_lm": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _f, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                   _vp, _vp, _i64, _i32, _i32, _f, _vp]),
     "st5_beam_update": (C.c_int, [_i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _f] + [_vp] * 18),
     "st5_attn_fused_fwd": (C.c_int, [C.POINTER(AttnArgs), _vp, _vp, _vp, _vp, _vp]),
     "st5_attn_flash_fwd": (C.c_int, [C.POINTER(AttnArgs), _vp, _vp, _vp, _vp, _vp]),

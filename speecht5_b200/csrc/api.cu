@@ -149,6 +149,15 @@ int st5_beam_topk(const void* logits, int64_t ld, int dtype, int32_t B, int32_t 
                                     cand_score, cand_token, cand_beam, ws, (cudaStream_t)stream),
                    "st5_beam_topk");
 }
+int st5_beam_topk_lm(const void* logits, int64_t ld, int dtype, int32_t B, int32_t K, int32_t V, const float* cum,
+                     const float* mask, float inv_temp, int32_t eos, const int64_t* t, const int64_t* min_len,
+                     const int64_t* max_len, float* cand_score, int32_t* cand_token, int32_t* cand_beam, float* ws,
+                     const void* lm_logits, int64_t lm_ld, int lm_dtype, int32_t V_lm, float lm_weight, void* stream) {
+  return set_error(beam_topk_lm_launch(logits, ld, dtype, B, K, V, cum, mask, inv_temp, eos, t, min_len, max_len,
+                                       lm_logits, lm_ld, lm_dtype, V_lm, lm_weight, cand_score, cand_token, cand_beam,
+                                       ws, (cudaStream_t)stream),
+                   "st5_beam_topk_lm");
+}
 int st5_beam_update(int32_t B, int32_t K, int32_t V, int32_t T, int32_t eos, const int64_t* t, const int64_t* max_len,
                     int32_t normalize, float len_penalty, const float* cand_score, const int32_t* cand_token,
                     const int32_t* cand_beam, int32_t* lin, int32_t* tok, float* score, int32_t* ignore,

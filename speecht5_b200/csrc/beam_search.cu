@@ -1,8 +1,8 @@
 // Beam search over the text decoder's vocabulary: candidate selection and the per-sentence bookkeeping of one step.
 //
 // Reference: speecht5/sequence_generator.py:430-636 (score masking, search.step, finalize, active-hypothesis selection)
-// with finalize_hypos / is_finished (:690-816) and fairseq/search.py:117-144 (BeamSearch.step), ctc_weight 0, no LM,
-// no prefix tokens.
+// with finalize_hypos / is_finished (:690-816) and fairseq/search.py:117-144 (BeamSearch.step), ctc_weight 0, no prefix
+// tokens; with or without a language model's log-probabilities added before the masking (:420-426).
 //
 // Candidate selection is exact: each row's top n (the sentence needs n = min(2K, F - 1)) is found by n rounds of a
 // CTA-wide arg-max over the row's masked log-probabilities, each round taking the best element strictly after the
@@ -48,12 +48,39 @@ __device__ __forceinline__ int beam_n(int t, int K, int V) {
   return min(2 * K, F - 1);
 }
 
-template <typename T>
-__global__ void __launch_bounds__(BT) beam_row_topk(const T* logits, int64_t ld, int K, int V, const float* cum,
-                                                    const float* mask, float inv_temp, int eos, const int64_t* tp,
-                                                    const int64_t* minp, const int64_t* maxp, float* ws) {
-  __shared__ float red[BT / 32];
-  __shared__ Cand best[BT / 32];
+// the language model's row of a fused step (sequence_generator.py:420-426): logits y[r * ld + v] for v < V
+struct LmRow {
+  const void* y;
+  int64_t ld;
+  int dtype;
+  int V;
+  float w;
+};
+
+__device__ __forceinline__ float lm_ld(const LmRow& lm, int64_t i) {
+  return lm.dtype == ST5_F32 ? ldf(static_cast<const float*>(lm.y) + i)
+                             : ldf(static_cast<const __nv_bfloat16*>(lm.y) + i);
+}
+
+// CTA-wide max (sum when !MAX) of one value per thread; every thread gets the result
+template <bool MAX>
+__device__ __forceinline__ float cta_reduce(float v, float (&red)[BT / 32], int lane, int w) {
+  v = MAX ? warp_max(v) : warp_sum(v);
+  if (lane == 0) red[w] = v;
+  __syncthreads();
+  v = MAX ? red[0] : 0.f;
+#pragma unroll
+  for (int i = MAX ? 1 : 0; i < BT / 32; ++i) v = MAX ? fmaxf(v, red[i]) : v + red[i];
+  __syncthreads();
+  return v;
+}
+
+// one CTA per row: the row's best n candidates into ws; with LM the row's score gains lm.w * log_softmax(y)[v], v < lm.V
+template <typename T, bool LM>
+__device__ __forceinline__ void row_topk(const T* logits, int64_t ld, int K, int V, const float* cum, const float* mask,
+                                         float inv_temp, int eos, const int64_t* tp, const int64_t* minp,
+                                         const int64_t* maxp, float* ws, float (&red)[BT / 32], Cand (&best)[BT / 32],
+                                         const LmRow lm) {
   const int r = blockIdx.x, tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int64_t t = *tp;
   if (t == 0 && r % K != 0) return;  // (search.py:119-122: step 0 reads beam 0 only)
@@ -77,6 +104,18 @@ __global__ void __launch_bounds__(BT) beam_row_topk(const T* logits, int64_t ld,
 #pragma unroll
   for (int i = 0; i < BT / 32; ++i) l += red[i];
   const float lse = logf(l);
+  // the LM's log-softmax over its own vocabulary, in fp32, without the temperature (:420-425)
+  float ym = 0.f, ylse = 0.f;
+  if constexpr (LM) {
+    const int64_t yo = (int64_t)r * lm.ld;
+    __syncthreads();  // (red is reused)
+    ym = -INFINITY;
+    for (int v = tid; v < lm.V; v += BT) ym = fmaxf(ym, lm_ld(lm, yo + v));
+    ym = cta_reduce<true>(ym, red, lane, w);
+    float yl = 0.f;
+    for (int v = tid; v < lm.V; v += BT) yl += expf(lm_ld(lm, yo + v) - ym);
+    ylse = logf(cta_reduce<false>(yl, red, lane, w));
+  }
   const bool no_eos = t < *minp, only_eos = t >= *maxp;
   const float c0 = t > 0 ? cum[r] : 0.f;
   float* ws_s = ws + (int64_t)r * 2 * BKMAX * 2;
@@ -87,6 +126,9 @@ __global__ void __launch_bounds__(BT) beam_row_topk(const T* logits, int64_t ld,
     Cand c{-INFINITY, 0x7fffffff};
     for (int v = tid; v < V; v += BT) {
       float lp = (ldf(x + v) * inv_temp - m) - lse;
+      if constexpr (LM) {
+        if (v < lm.V) lp += lm.w * ((lm_ld(lm, (int64_t)r * lm.ld + v) - ym) - ylse);  // (:426, before any masking)
+      }
       if (no_eos && v == eos) lp = -INFINITY;
       if (lp != lp) lp = -INFINITY;
       lp += mask[v];
@@ -109,6 +151,25 @@ __global__ void __launch_bounds__(BT) beam_row_topk(const T* logits, int64_t ld,
     ps = c.s;
     pi = c.i;
   }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(BT) beam_row_topk(const T* logits, int64_t ld, int K, int V, const float* cum,
+                                                    const float* mask, float inv_temp, int eos, const int64_t* tp,
+                                                    const int64_t* minp, const int64_t* maxp, float* ws) {
+  __shared__ float red[BT / 32];
+  __shared__ Cand best[BT / 32];
+  row_topk<T, false>(logits, ld, K, V, cum, mask, inv_temp, eos, tp, minp, maxp, ws, red, best, LmRow{});
+}
+
+template <typename T>
+__global__ void __launch_bounds__(BT) lm_fused_row_topk(const T* logits, int64_t ld, int K, int V, const float* cum,
+                                                        const float* mask, float inv_temp, int eos, const int64_t* tp,
+                                                        const int64_t* minp, const int64_t* maxp, float* ws,
+                                                        const LmRow lm) {
+  __shared__ float red[BT / 32];
+  __shared__ Cand best[BT / 32];
+  row_topk<T, true>(logits, ld, K, V, cum, mask, inv_temp, eos, tp, minp, maxp, ws, red, best, lm);
 }
 
 // one warp per sentence: the best n of the union of its rows' lists, flat index beam * V + token
@@ -269,6 +330,29 @@ int beam_topk_launch(const void* logits, int64_t ld, int dtype, int B, int K, in
   else
     beam_row_topk<__nv_bfloat16><<<B * K, BT, 0, st>>>((const __nv_bfloat16*)logits, ld, K, V, cum, mask, inv_temp,
                                                       eos, t, min_len, max_len, ws);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return (int)e;
+  beam_merge_topk<<<B, 32, 0, st>>>(K, V, t, ws, cand_score, cand_token, cand_beam);
+  return (int)cudaGetLastError();
+}
+
+int beam_topk_lm_launch(const void* logits, int64_t ld, int dtype, int B, int K, int V, const float* cum,
+                        const float* mask, float inv_temp, int eos, const int64_t* t, const int64_t* min_len,
+                        const int64_t* max_len, const void* lm_logits, int64_t lm_ld, int lm_dtype, int V_lm,
+                        float lm_weight, float* cand_score, int32_t* cand_token, int32_t* cand_beam, float* ws,
+                        cudaStream_t st) {
+  if (B <= 0 || K < 1 || K > BKMAX || V < 2 || V > BVMAX || eos < 0 || eos >= V || V_lm < 1 || V_lm > V) return -2;
+  if (!logits || !cum || !mask || !t || !min_len || !max_len || !lm_logits || !cand_score || !cand_token ||
+      !cand_beam || !ws)
+    return -3;
+  if (ld < V || lm_ld < V_lm) return -6;
+  const LmRow lm{lm_logits, lm_ld, lm_dtype, V_lm, lm_weight};
+  if (dtype == ST5_F32)
+    lm_fused_row_topk<float><<<B * K, BT, 0, st>>>((const float*)logits, ld, K, V, cum, mask, inv_temp, eos, t,
+                                                   min_len, max_len, ws, lm);
+  else
+    lm_fused_row_topk<__nv_bfloat16><<<B * K, BT, 0, st>>>((const __nv_bfloat16*)logits, ld, K, V, cum, mask,
+                                                           inv_temp, eos, t, min_len, max_len, ws, lm);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
   beam_merge_topk<<<B, 32, 0, st>>>(K, V, t, ws, cand_score, cand_token, cand_beam);

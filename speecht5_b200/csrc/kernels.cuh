@@ -153,6 +153,11 @@ int beam_topk_launch(const void* logits, int64_t ld, int dtype, int B, int K, in
                      const float* mask, float inv_temp, int eos, const int64_t* t, const int64_t* min_len,
                      const int64_t* max_len, float* cand_score, int32_t* cand_token, int32_t* cand_beam, float* ws,
                      cudaStream_t s);
+int beam_topk_lm_launch(const void* logits, int64_t ld, int dtype, int B, int K, int V, const float* cum,
+                        const float* mask, float inv_temp, int eos, const int64_t* t, const int64_t* min_len,
+                        const int64_t* max_len, const void* lm_logits, int64_t lm_ld, int lm_dtype, int V_lm,
+                        float lm_weight, float* cand_score, int32_t* cand_token, int32_t* cand_beam, float* ws,
+                        cudaStream_t s);
 int beam_update_launch(int B, int K, int V, int T, int eos, const int64_t* t, const int64_t* max_len, int normalize,
                        float len_penalty, const float* cand_score, const int32_t* cand_token, const int32_t* cand_beam,
                        int32_t* lin, int32_t* tok, float* score, int32_t* ignore, int32_t* finished, int32_t* parent,

@@ -97,6 +97,11 @@ def decoder_step(decoder, x_new, cache, need_head_weights=False, t_dev=None, spa
         else:
             x = ops.residual_layer_norm(ops.linear(a, sa.out_proj.weight, sa.out_proj.bias), residual,
                                         layer.self_attn_layer_norm)
+        if ca is None:  # a decoder without encoder attention (the fusion LM, lm.TransformerLM): pre-LN only
+            assert layer.normalize_before
+            x = ops.ffn(ops.residual_layer_norm(x, None, layer.final_layer_norm), layer.fc1, layer.fc2,
+                        layer.activation_fn, residual=x)
+            continue
         residual = x
         h = ops.residual_layer_norm(x, None, layer.encoder_attn_layer_norm) if layer.normalize_before else x
         q = ops.linear(h, ca.q_proj.weight, ca.q_proj.bias)
@@ -505,11 +510,17 @@ class BeamGraph:
     key/value cache: each (row, position) cell is written once, and the lineage table lin[row][position] -- the
     self-attention's kv_rows -- says which row's cell holds each position of a hypothesis. Cross keys / values are
     projected once per sentence into [B, S, 2C]; the K beams read them with kv_div = K. Utterance-independent like
-    GreedyGraph: encoder length and step budget are buckets. capture=False runs the same step body eagerly."""
+    GreedyGraph: encoder length and step budget are buckets. capture=False runs the same step body eagerly.
+
+    With a language model `lm` (lm.TransformerLM, shallow fusion :420-426) the same replay also runs the LM one position
+    per row -- embedding + position of the newest token, its layers on a [B*K, rows, 2C_lm] key/value cache per layer,
+    its output projection -- and st5_beam_topk_lm adds lm_weight * log_softmax(LM logits) before the masking. The LM's
+    cells are written once per (row, position) and read through the same lineage table, so a reorder moves no LM cache
+    either. Token 0 of every hypothesis is eos for the LM as for the decoder."""
 
     CHUNK = 8
 
-    def __init__(self, model, B, K, S_bucket, maxlen_bucket, device, capture=True):
+    def __init__(self, model, B, K, S_bucket, maxlen_bucket, device, capture=True, lm=None):
         self.m, self.capture = model, capture
         dec = model.decoder
         dev = torch.device(device)
@@ -538,14 +549,22 @@ class BeamGraph:
         self.mask = torch.zeros(self.V, dtype=torch.float32, device=dev)  # pad / blank / mask symbol never, unk penalty
         self.pos = torch.arange(rows, device=dev)
         self.pe = model.text_decoder_prenet._table(rows, dev)
-        self.consts = None  # (eos, 1 / temperature, normalize, len_penalty): host arguments the graphs bake
+        self.lm = lm
+        if lm is not None:
+            C_lm = lm.args.decoder_embed_dim
+            self.lm_cache = _StaticCache([], [torch.zeros((BK, rows, 2 * C_lm), dtype=RT.dtype, device=dev)
+                                              for _ in lm.decoder.layers], None, rows)
+            self.lm_emb = torch.zeros((lm.vocab_size, C_lm), dtype=torch.float32, device=dev)  # embed_scale * E
+            self.lm_pe = torch.zeros((rows, C_lm), dtype=torch.float32, device=dev)
+        # (eos, 1 / temperature, normalize, len_penalty, lm_weight): host arguments the graphs bake
+        self.consts = None
         self.graphs = {}
         self.stream = torch.cuda.Stream(device=dev) if capture else None
         self.dtype = RT.dtype
 
     @torch.no_grad()
     def begin(self, encoder_out, max_len, min_len, unk_penalty, temperature, pad, eos, unk, blank, mask_idx,
-              normalize_scores, len_penalty):
+              normalize_scores, len_penalty, lm_weight=0.0):
         import math
         enc = encoder_out.get("_encoder_out_btc")
         if enc is None:
@@ -567,7 +586,12 @@ class BeamGraph:
         self.mask[blank] = -math.inf
         if mask_idx is not None and mask_idx != unk:
             self.mask[mask_idx] = -math.inf
-        consts = (int(eos), 1.0 / float(temperature), bool(normalize_scores), float(len_penalty))
+        if self.lm is not None:  # (the tables the LM's graph body reads: refreshed for weights changed in place)
+            self.lm_emb.copy_(self.lm.scaled_embedding())
+            n = min(self.lm_pe.shape[0], max_len + 1)  # (positions past the step budget are never read)
+            self.lm_pe.zero_()
+            self.lm_pe[:n] = self.lm.positions(n, self.dev)
+        consts = (int(eos), 1.0 / float(temperature), bool(normalize_scores), float(len_penalty), float(lm_weight))
         if self.graphs and consts != self.consts:
             self.graphs = {}
         self.consts = consts
@@ -581,7 +605,7 @@ class BeamGraph:
 
     def _body(self, span):
         m, pre, st = self.m, self.m.text_decoder_prenet, self.state
-        eos, inv_temp, normalize, len_penalty = self.consts
+        eos, inv_temp, normalize, len_penalty, lm_weight = self.consts
         BK = self.B * self.K
         x = ops.scaled_posenc(self.pe.index_select(0, self.t), pre._unit, 0.0, tokens=st["cur_tok"].view(BK, 1),
                               emb=pre.embed_tokens.weight, padding_idx=pre.padding_idx)
@@ -589,8 +613,15 @@ class BeamGraph:
         z, _ = decoder_step(m.decoder, x, self.cache, t_dev=self.t, span=span, self_pad=self_pad, self_rows=st["lin"],
                             cross_div=self.K)
         logits = m.text_decoder_postnet(z)
+        fusion = {}  # (without an LM: st5_beam_topk)
+        if self.lm is not None:
+            y = ops.scaled_posenc(self.lm_pe.index_select(0, self.t), self.lm._unit, 0.0,
+                                  tokens=st["cur_tok"].view(BK, 1), emb=self.lm_emb, padding_idx=self.lm.padding_idx)
+            zl, _ = decoder_step(self.lm.decoder, y, self.lm_cache, t_dev=self.t, span=span, self_pad=self_pad,
+                                 self_rows=st["lin"])
+            fusion = dict(lm_logits=self.lm.output_layer(zl)[:, -1, :], lm_weight=lm_weight)
         kernels.beam_topk(logits[:, -1, :], st["cur_score"], self.mask, inv_temp, eos, self.t, self.min_len,
-                          st["max_len"], st["cand_score"], st["cand_token"], st["cand_beam"], K=self.K)
+                          st["max_len"], st["cand_score"], st["cand_token"], st["cand_beam"], K=self.K, **fusion)
         kernels.beam_update(st, K=self.K, V=self.V, eos=eos, normalize=normalize, len_penalty=len_penalty)
         self.t += 1
 
@@ -632,18 +663,19 @@ class BeamGraph:
         return out
 
 
-def beam_graph(model, B, K, S, max_len, device, capture=True):
+def beam_graph(model, B, K, S, max_len, device, capture=True, lm=None):
     """The model's BeamGraph for B sentences x K beams, encoder length S and max_len steps (buckets: S to multiples of
-    64, max_len to powers of two >= 64); rebuilt when the numeric mode or the weights changed."""
+    64, max_len to powers of two >= 64), fused with the language model `lm` or none; rebuilt when the numeric mode or
+    the weights changed."""
     S_b = max(64, (S + 63) // 64 * 64)
     M_b = 64
     while M_b < max_len:
         M_b *= 2
     store = model.__dict__.setdefault("_beam_graphs", {})
-    key = (B, K, S_b, M_b, RT.dtype, str(device), bool(capture), RT.param_epoch)
+    key = (B, K, S_b, M_b, RT.dtype, str(device), bool(capture), None if lm is None else id(lm), RT.param_epoch)
     bg = store.get(key)
     if bg is None:
-        for k in [k for k in store if k[:7] == key[:7]]:
+        for k in [k for k in store if k[:8] == key[:8]]:
             del store[k]
-        bg = store[key] = BeamGraph(model, B, K, S_b, M_b, device, capture=capture)
+        bg = store[key] = BeamGraph(model, B, K, S_b, M_b, device, capture=capture, lm=lm)
     return bg

@@ -240,10 +240,13 @@ def attn_lineage_fwd(q, k, v, out, *, H, scale, key_pad=None, kv_rows=None, kv_d
     _count(1 if nws == 0 else 2)
 
 
-def beam_topk(logits, cum, mask, inv_temp, eos, t, min_len, max_len, cand_score, cand_token, cand_beam, *, K):
+def beam_topk(logits, cum, mask, inv_temp, eos, t, min_len, max_len, cand_score, cand_token, cand_beam, *, K,
+              lm_logits=None, lm_weight=0.0):
     """st5_beam_topk: logits [B*K, V] (row pitch logits.stride(0), fp32 / bf16), cum [B*K] fp32, mask [V] fp32; t /
-    min_len / max_len int64 device scalars; cand_* [B, 2K] (fp32, int32, int32) receive the first min(2K, F-1)."""
-    _require_cuda(logits, cum, mask, t, min_len, max_len, cand_score, cand_token, cand_beam)
+    min_len / max_len int64 device scalars; cand_* [B, 2K] (fp32, int32, int32) receive the first min(2K, F-1).
+    With lm_logits [B*K, V_lm] (V_lm <= V, fp32 / bf16, row pitch lm_logits.stride(0)): st5_beam_topk_lm, which adds
+    lm_weight * log_softmax(lm_logits) to the first V_lm log-probabilities before the masking."""
+    _require_cuda(logits, cum, mask, t, min_len, max_len, cand_score, cand_token, cand_beam, lm_logits)
     assert logits.stride(1) == 1 and cum.dtype == torch.float32 and mask.dtype == torch.float32
     assert t.dtype == min_len.dtype == max_len.dtype == torch.int64
     assert cand_score.dtype == torch.float32 and cand_token.dtype == cand_beam.dtype == torch.int32
@@ -251,9 +254,16 @@ def beam_topk(logits, cum, mask, inv_temp, eos, t, min_len, max_len, cand_score,
     B = BK // K
     lib = _lib.load()
     ws = torch.empty(max(1, lib.st5_beam_topk_ws_floats(B, K)), dtype=torch.float32, device=logits.device)
-    _lib.check(lib.st5_beam_topk(_ptr(logits), logits.stride(0), dtype_id(logits), B, K, V, _ptr(cum), _ptr(mask),
-                                 float(inv_temp), int(eos), _ptr(t), _ptr(min_len), _ptr(max_len), _ptr(cand_score),
-                                 _ptr(cand_token), _ptr(cand_beam), _ptr(ws), _stream()), "st5_beam_topk")
+    args = (_ptr(logits), logits.stride(0), dtype_id(logits), B, K, V, _ptr(cum), _ptr(mask), float(inv_temp), int(eos),
+            _ptr(t), _ptr(min_len), _ptr(max_len), _ptr(cand_score), _ptr(cand_token), _ptr(cand_beam), _ptr(ws))
+    if lm_logits is None:
+        _lib.check(lib.st5_beam_topk(*args, _stream()), "st5_beam_topk")
+    else:
+        assert lm_logits.stride(1) == 1 and lm_logits.shape[0] == BK
+        if lm_logits.shape[1] > V:
+            raise ValueError(f"the LM vocabulary ({lm_logits.shape[1]}) is larger than the decoder's ({V})")
+        _lib.check(lib.st5_beam_topk_lm(*args, _ptr(lm_logits), lm_logits.stride(0), dtype_id(lm_logits),
+                                        lm_logits.shape[1], float(lm_weight), _stream()), "st5_beam_topk_lm")
     _count(2)
 
 

@@ -554,14 +554,18 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
     @torch.no_grad()
     def generate_text_beam(self, source, padding_mask=None, beam_size=5, max_len_a=0.0, max_len_b=200, min_len=1,
                            unk_penalty=0.0, temperature=1.0, pad=1, eos=2, unk=3, blank=0, mask_idx=None, use_cache=True,
-                           normalize_scores=True, len_penalty=1.0):
+                           normalize_scores=True, len_penalty=1.0, lm=None, lm_weight=1.0):
         """Beam search as `generate.py --beam K` runs it (speecht5/sequence_generator.py:207-654 with ctc_weight 0, no
-        LM, no prefix tokens): the masking of generate_text_greedy, the best 2K candidates of each sentence per step
+        prefix tokens): the masking of generate_text_greedy, the best 2K candidates of each sentence per step
         (fairseq/search.py:117-144), hypotheses finalized at eos until K are held or max_len is reached. beam_size is
         clamped to V - 1 (:99); max_len as in generate_text_greedy. Returns per sentence its K hypotheses sorted by score
         descending, {"tokens", "score", "attention": None, "alignment", "positional_scores"} (:644-654).
         use_cache: True (key/value cache, the step body run eagerly) or "graph" (one captured CUDA graph per step);
-        both on speecht5_b200/incremental.BeamGraph."""
+        both on speecht5_b200/incremental.BeamGraph.
+        lm: a language model for shallow fusion (`--lm-path`, :420-426), a speecht5_b200.lm.TransformerLM
+        (TransformerLM.from_fairseq converts the fairseq transformer_lm generate.py loads), whose log-probabilities
+        times lm_weight are added to the first V_lm entries of every step's log-probabilities before the masking
+        (V_lm <= V; the ASR dictionary's <mask> and <ctc_blank> usually lie past the LM's vocabulary)."""
         if use_cache not in (True, "graph"):
             raise ValueError(f"generate_text_beam: use_cache must be True or 'graph', got {use_cache!r}")
         B, src_len = source.size(0), source.size(1)
@@ -569,12 +573,22 @@ class T5TransformerModel(FairseqEncoderDecoderModel):
         assert min_len <= max_len
         V = self.text_decoder_postnet.output_projection.weight.shape[0]
         K = min(int(beam_size), V - 1)
+        if lm is not None:
+            from ..lm import TransformerLM
+            if not isinstance(lm, TransformerLM):
+                raise TypeError("generate_text_beam: lm must be a speecht5_b200.lm.TransformerLM "
+                                "(TransformerLM.from_fairseq converts a fairseq transformer_lm)")
+            if lm.vocab_size > V:
+                raise ValueError(f"generate_text_beam: the LM vocabulary ({lm.vocab_size}) is larger than the "
+                                 f"decoder's ({V})")
+            lm.positions(max_len + 1, "cpu")  # (learned positions must cover the step budget)
         enc = self.forward_encoder(source, padding_mask=padding_mask)
         from ..incremental import beam_graph
-        bg = beam_graph(self, B, K, enc["encoder_out"][0].size(0), max_len, source.device, capture=use_cache == "graph")
+        bg = beam_graph(self, B, K, enc["encoder_out"][0].size(0), max_len, source.device, capture=use_cache == "graph",
+                        lm=lm)
         return bg.decode(enc, max_len, min_len=min_len, unk_penalty=unk_penalty, temperature=temperature, pad=pad,
                          eos=eos, unk=unk, blank=blank, mask_idx=mask_idx, normalize_scores=normalize_scores,
-                         len_penalty=len_penalty)
+                         len_penalty=len_penalty, lm_weight=lm_weight if lm is not None else 0.0)
 
     def forward_text_encoder(self, src_tokens):
         encoder_input, encoder_padding_mask = self.text_encoder_prenet(src_tokens)

@@ -3,7 +3,10 @@
 beam-1 GreedyGraph on the same inputs. The number of steps is fixed with min_len = max_len (eos is banned until the last
 step, where it is the only choice), so an untrained model's outputs do not change the timing. Encoder included.
 
-Also CUDA-event times of st5_beam_topk and st5_beam_update alone (V = 81 and V = 8 000, the ASR character and the
+With --lm, the same beam rows again with LM shallow fusion (`lm=`, `lm_weight` 0.5): a random-weight fairseq
+transformer_lm of base size (6 layers x 512, 8 heads, FFN 2048, vocabulary V - 2) run inside every captured step.
+
+Also CUDA-event times of st5_beam_topk (and, with --lm, st5_beam_topk_lm at V_lm = V - 2) and st5_beam_update alone (V = 81 and V = 8 000, the ASR character and the
 MuST-C ST vocabularies) and of st5_attn_lineage_fwd at the 10 s cross-attention shape (8 sentences x K beams over one
 copy of 500 encoder keys per sentence, 12 heads), with bytes per second from shapes.
 Prints one JSON line with the card's name and power limit."""
@@ -38,6 +41,7 @@ def card():
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=64, help="decoder steps per decode (min_len = max_len)")
+    ap.add_argument("--lm", action="store_true", help="also the LM-fusion rows")
     args = ap.parse_args()
     import torch
     from speecht5_b200 import kernels
@@ -64,6 +68,19 @@ def main():
         ms1 = cuda_ms(lambda: asr.generate_text_beam(wav[:1], wpm[:1], beam_size=K, use_cache="graph", **kw))
         out[f"beam{K}_graph"] = dict(ms_B8=ms8, ms_per_step_B8=ms8 / (n + 1), utt_per_s_B8=8 / (ms8 / 1e3), ms_B1=ms1,
                                      ms_per_step_B1=ms1 / (n + 1), speedup_B8_over_8x_B1=8 * ms1 / ms8)
+    if args.lm:
+        from argparse import Namespace
+        from speecht5_b200.lm import TransformerLM
+        V = asr.text_decoder_postnet.output_projection.weight.shape[0]
+        lm = TransformerLM(Namespace(decoder_layers=6, decoder_embed_dim=512, decoder_attention_heads=8,
+                                     decoder_ffn_embed_dim=2048), V - 2)
+        for p in lm.parameters():
+            torch.nn.init.normal_(p, std=0.05)
+        lm = lm.to(dev)
+        for K in (5, 10):
+            ms8 = cuda_ms(lambda: asr.generate_text_beam(wav, wpm, beam_size=K, use_cache="graph", lm=lm, lm_weight=0.5,
+                                                         **kw))
+            out[f"beam{K}_lm_graph"] = dict(ms_B8=ms8, ms_per_step_B8=ms8 / (n + 1), utt_per_s_B8=8 / (ms8 / 1e3))
     del asr
     # kernels alone
     B, t = 8, torch.tensor([5], dtype=torch.int64, device=dev)
@@ -76,6 +93,11 @@ def main():
             ct, cb = (torch.empty(B, 2 * K, dtype=torch.int32, device=dev) for _ in range(2))
             us = 1e3 * cuda_ms(lambda: kernels.beam_topk(logits, cum, mask, 1.0, 2, t, mn, mx, cs, ct, cb, K=K), reps=200)
             out[f"beam_topk_V{V}_K{K}_us"] = us
+            if args.lm:
+                lm_logits = torch.randn(B * K, V - 2, device=dev)
+                us = 1e3 * cuda_ms(lambda: kernels.beam_topk(logits, cum, mask, 1.0, 2, t, mn, mx, cs, ct, cb, K=K,
+                                                             lm_logits=lm_logits, lm_weight=0.5), reps=200)
+                out[f"beam_topk_lm_V{V}_K{K}_us"] = us
     for K in (5, 10):
         T = 73
         i32, f32 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.float32, device=dev)
