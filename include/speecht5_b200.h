@@ -133,6 +133,14 @@ int st5_ln_bwd(const void* dy, const void* s, const float* mean, const float* rs
  * one pass. x [B, T, C], out [B, n_in, C], C a multiple of 8; slope = 1 copies. */
 int st5_lrelu_pad(const void* x, void* out, int64_t B, int64_t T, int64_t C, int64_t n_in, int32_t d, int32_t ph,
                   int32_t pad, float slope, void* stream);
+/* st5_lrelu_pad over a padded batch of ragged utterances: source frames are limited to [0, L_b) with
+ * L_b = clamp(lengths[b] * len_mult, 0, T) (int64), so row b is staged exactly as utterance b alone would be, and x is
+ * never read at or past L_b. lengths: int32 [B] in device memory (a captured graph replays for any lengths; NULL:
+ * L_b = T, i.e. st5_lrelu_pad); len_mult: the up-sampling factor between the lengths' resolution and x's.
+ * Returns -2 for C % 8 != 0, d < 1, ph outside [0, d), len_mult < 1 or the shape / alignment errors of st5_lrelu_pad;
+ * -3 for a NULL x or out. Nothing is launched on an error. */
+int st5_lrelu_pad_len(const void* x, void* out, int64_t B, int64_t T, int64_t C, int64_t n_in, int32_t d, int32_t ph,
+                      int32_t pad, float slope, const int32_t* lengths, int32_t len_mult, void* stream);
 
 /* y = dropout(x) (also its own backward when applied to the gradient). fairseq/modules/fairseq_dropout.py:23-37
  * (F.dropout semantics: keep with probability 1-p, scale by 1/(1-p)); mask = the counter-based generator above. */

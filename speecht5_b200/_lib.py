@@ -77,6 +77,7 @@ _PROTOS = {
     "st5_ln_bwd_blocks": (C.c_int64, [_i64]),
     "st5_ln_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _f, _u64, _u64, _vp]),
     "st5_lrelu_pad": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _f, _vp]),
+    "st5_lrelu_pad_len": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _f, _vp, _i32, _vp]),
     "st5_dropout": (C.c_int, [_vp, _vp, _i32, _i64, _f, _u64, _u64, _vp]),
     "st5_act_bwd": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i64, _f, _u64, _u64, _vp]),
     "st5_colsum": (C.c_int, [_vp, _i64, _vp, _i32, _i64, _i64, _i64, _i32, _vp]),

@@ -106,7 +106,13 @@ int st5_ln_bwd(const void* dy, const void* s, const float* mean, const float* rs
 
 int st5_lrelu_pad(const void* x, void* out, int64_t B, int64_t T, int64_t C, int64_t n_in, int32_t d, int32_t ph,
                   int32_t pad, float slope, void* stream) {
-  return set_error(lrelu_pad_launch(x, out, B, T, C, n_in, d, ph, pad, slope, (cudaStream_t)stream), "st5_lrelu_pad");
+  return set_error(lrelu_pad_launch(x, out, B, T, C, n_in, d, ph, pad, slope, nullptr, 1, (cudaStream_t)stream),
+                   "st5_lrelu_pad");
+}
+int st5_lrelu_pad_len(const void* x, void* out, int64_t B, int64_t T, int64_t C, int64_t n_in, int32_t d, int32_t ph,
+                      int32_t pad, float slope, const int32_t* lengths, int32_t len_mult, void* stream) {
+  return set_error(lrelu_pad_launch(x, out, B, T, C, n_in, d, ph, pad, slope, lengths, len_mult, (cudaStream_t)stream),
+                   "st5_lrelu_pad_len");
 }
 
 int st5_dropout(const void* x, void* y, int dtype, int64_t n, float drop_p, uint64_t seed, uint64_t offset,

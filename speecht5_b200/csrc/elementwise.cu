@@ -205,18 +205,28 @@ int posenc_bwd_launch(const void* dy, const int64_t* tokens, int64_t padding_idx
 // ------------------------------------------------------------------ leaky-ReLU into a padded / de-interleaved operand
 // HiFi-GAN (SpeechUT/.../hifigan.py:70-100,154-170): every convolution is preceded by a leaky-ReLU and consumed here as a
 // window GEMM over a zero-padded copy of its input; dilated convolutions read one PHASE (frames ph, ph+d, ...) of it.
-// out[b][m][:] = lrelu(x[b][ph + d*m - pad][:]) for frames inside [0, T), zeros outside: one pass instead of the
+// out[b][m][:] = lrelu(x[b][ph + d*m - pad][:]) for frames inside [0, L_b), zeros outside: one pass instead of the
 // activation, the zero fill and the strided copy (three launches, two extra round trips of the activations).
+// L_b = clamp(lengths[b] * len_mult, 0, T) (lengths == nullptr: T), so one padded batch of ragged utterances stages
+// each utterance exactly as it would be staged alone; frames at or past L_b are never read. LEN = false (no lengths)
+// compiles the length test out: st5_lrelu_pad's hot path stays the kernel it was.
+template <bool LEN>
 __global__ void lrelu_pad_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ out, int64_t B,
-                                 int64_t T, int64_t C, int64_t n_in, int d, int ph, int pad, float slope) {
+                                 int64_t T, int64_t C, int64_t n_in, int d, int ph, int pad, float slope,
+                                 const int32_t* __restrict__ lengths, int len_mult) {
   pdl_sync();
   const int64_t cpr = C >> 3, n8 = B * n_in * cpr;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n8; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t row = i / cpr, c = (i - row * cpr) * 8;
     const int64_t b = row / n_in, m = row - b * n_in;
     const int64_t xi = (int64_t)ph + (int64_t)d * m - pad;
+    int64_t L = T;
+    if (LEN) {
+      const int64_t l = (int64_t)__ldg(lengths + b) * len_mult;
+      L = l < 0 ? 0 : (l < T ? l : T);
+    }
     uint4 o = make_uint4(0u, 0u, 0u, 0u);
-    if (xi >= 0 && xi < T) {
+    if (xi >= 0 && xi < L) {
       float v[8];
       load8<__nv_bfloat16>(x + (b * T + xi) * C + c, v);
 #pragma unroll
@@ -229,11 +239,14 @@ __global__ void lrelu_pad_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloa
   }
 }
 int lrelu_pad_launch(const void* x, void* out, int64_t B, int64_t T, int64_t C, int64_t n_in, int d, int ph, int pad,
-                     float slope, cudaStream_t s) {
-  if (B <= 0 || T <= 0 || C <= 0 || (C & 7) || n_in <= 0 || d <= 0 || ph < 0 || ph >= d || !aligned16(x) || !aligned16(out))
+                     float slope, const int32_t* lengths, int len_mult, cudaStream_t s) {
+  if (x == nullptr || out == nullptr) return -3;
+  if (B <= 0 || T <= 0 || C <= 0 || (C & 7) || n_in <= 0 || d <= 0 || ph < 0 || ph >= d || len_mult < 1 ||
+      !aligned16(x) || !aligned16(out))
     return -2;
-  launch_pdl(lrelu_pad_kernel, dim3(grid_for(B * n_in * (C >> 3), 256)), dim3(256), 0, s, (const __nv_bfloat16*)x,
-             (__nv_bfloat16*)out, B, T, C, n_in, d, ph, pad, slope);
+  launch_pdl(lengths != nullptr ? lrelu_pad_kernel<true> : lrelu_pad_kernel<false>,
+             dim3(grid_for(B * n_in * (C >> 3), 256)), dim3(256), 0, s, (const __nv_bfloat16*)x, (__nv_bfloat16*)out, B,
+             T, C, n_in, d, ph, pad, slope, lengths, len_mult);
   return (int)cudaGetLastError();
 }
 

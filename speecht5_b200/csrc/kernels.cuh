@@ -136,7 +136,7 @@ int ln_bwd_launch(const void* dy, const void* s_in, const float* mean, const flo
                   void* dx, float* dgamma, float* dbeta, float* dxsum, int dtype, int64_t rows, int64_t C,
                   float drop_p, uint64_t seed, uint64_t offset, cudaStream_t s);
 int lrelu_pad_launch(const void* x, void* out, int64_t B, int64_t T, int64_t C, int64_t n_in, int d, int ph, int pad,
-                     float slope, cudaStream_t s);
+                     float slope, const int32_t* lengths, int len_mult, cudaStream_t s);
 int dropout_launch(const void* x, void* y, int dtype, int64_t n, float drop_p, uint64_t seed, uint64_t offset,
                    cudaStream_t s);
 int act_bwd_launch(const void* dy, const void* pre, void* dpre, int dtype, int act, int64_t n, float drop_p,

@@ -158,6 +158,20 @@ def lrelu_pad(x, out, d, ph, pad, slope):
     _count(1)
 
 
+def lrelu_pad_len(x, out, d, ph, pad, slope, lengths, len_mult=1):
+    """st5_lrelu_pad_len: lrelu_pad with the source frames of row b limited to [0, clamp(lengths[b] * len_mult, 0, T));
+    lengths: int32 [B] device tensor (None: T for every row)."""
+    _require_cuda(x, out, lengths)
+    assert x.dtype == torch.bfloat16 and out.dtype == torch.bfloat16 and x.is_contiguous() and out.is_contiguous()
+    B, T, Cc = x.shape
+    assert out.shape[0] == B and out.shape[2] == Cc
+    assert lengths is None or (lengths.dtype == torch.int32 and lengths.is_contiguous() and lengths.numel() >= B)
+    _lib.check(_lib.load().st5_lrelu_pad_len(_ptr(x), _ptr(out), B, T, Cc, out.shape[1], int(d), int(ph), int(pad),
+                                             float(slope), _ptr(lengths), int(len_mult), _stream()),
+               "st5_lrelu_pad_len")
+    _count(1)
+
+
 def dropout(x, y, drop_p, seed, offset):
     lib = _lib.load()
     _lib.check(lib.st5_dropout(_ptr(x), _ptr(y), dtype_id(x), x.numel(), drop_p, seed, offset, _stream()),

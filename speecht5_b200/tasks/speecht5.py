@@ -131,6 +131,24 @@ class SpeechT5Task(LegacyFairseqTask):
         args.update(kwargs)
         return models[0].generate_speech_batch(**args)
 
+    def generate_waveform_batch(self, models, net_input, vocoder, normalize_before=True, **kwargs):
+        """Speech out of a batch: generate_speech_batch (same net_input and keywords), then every utterance's mel through
+        `vocoder` (a speecht5_b200.vocoder.HifiGanGenerator) in one vocode call. Returns one (waveform [L_b * hop],
+        mel [L_b, odim], stop probabilities, attention or None) per utterance; mel and what follows it are exactly
+        generate_speech_batch's. The input is checked on the host before anything runs (ValueError)."""
+        key = "source" if "source" in net_input else "src_tokens"
+        x = net_input.get(key)
+        if not torch.is_tensor(x) or x.dim() != 2 or x.size(0) == 0 or x.size(1) == 0:
+            raise ValueError(f"net_input[{key!r}] must be a non-empty [B, T] tensor")
+        if x.device != vocoder.device:
+            raise ValueError(f"net_input is on {x.device}, the vocoder on {vocoder.device}")
+        odim = models[0].speech_decoder_postnet.odim
+        if vocoder.cfg["model_in_dim"] != odim:
+            raise ValueError(f"the vocoder takes {vocoder.cfg['model_in_dim']} mel channels, the model writes {odim}")
+        res = self.generate_speech_batch(models, net_input, **kwargs)
+        wavs = vocoder.vocode([mel for mel, _, _ in res], normalize_before)
+        return [(w, mel, probs, attn) for w, (mel, probs, attn) in zip(wavs, res)]
+
     def generate_class(self, models, net_input, prefix_tokens, **kwargs):
         """tasks/speecht5.py:631-638 (what scripts/generate_class.py calls): the predicted class of every utterance."""
         with torch.no_grad():

@@ -12,7 +12,14 @@ emulator against oracle/audio_oracle.py:HifiGanGenerator (tests/test_frontend_cp
 * dilated Conv1d(dilation d): the leaky-ReLU that precedes it writes its result de-interleaved into d phase buffers
   (frame t -> phase t mod d); inside a phase the dilation is 1, and each phase GEMM writes its rows back with pitch d*C.
 The leaky-ReLU, the zero padding and the de-interleave of every convolution input are ONE launch (st5_lrelu_pad); the
-ResBlock averaging is a torch elementwise call."""
+ResBlock averaging is a torch elementwise call.
+
+Ragged batches (`HifiGanGenerator.vocode`): the utterances are padded to one length and every operand staging takes the
+utterance's length at the current resolution (st5_lrelu_pad_len), so each convolution reads zeros past an utterance's
+end exactly as it does when the utterance is vocoded alone; every other step is row-independent (the GEMM rows, the
+epilogue, the elementwise calls). The whole pass is one captured CUDA graph per (batch, length bucket)."""
+import math
+
 import torch
 import torch.nn.functional as F
 
@@ -49,9 +56,18 @@ class _Conv:
         self.bias = bias.float().contiguous()
 
 
-def _conv_same(x, conv, out=None, act=None, residual=None, pre_act_slope=None):
+def _stage(x, buf, d, ph, pad, slope, lengths, len_mult):
+    if lengths is None:
+        K.lrelu_pad(x, buf, d, ph, pad, slope)
+    else:
+        K.lrelu_pad_len(x, buf, d, ph, pad, slope, lengths, len_mult)
+
+
+def _conv_same(x, conv, out=None, act=None, residual=None, pre_act_slope=None, lengths=None, len_mult=1):
     """'same' Conv1d on channels-last x [B, T, C_in] (bf16) -> [B, T, C_out]. pre_act_slope: leaky-ReLU applied to the
-    input while it is copied into the padded / de-interleaved operand buffer."""
+    input while it is copied into the padded / de-interleaved operand buffer. lengths (int32 [B] device tensor, times
+    len_mult = frames of x): frames of row b at or past its length are read as zeros, as if x ended there; the output
+    rows past it are then not meaningful."""
     B, T, Cin = x.shape
     k, d, Cout = conv.k, conv.d, conv.cout
     x = x.contiguous()
@@ -66,7 +82,7 @@ def _conv_same(x, conv, out=None, act=None, residual=None, pre_act_slope=None):
         # phase-frame i is padded index ph + d*i, i.e. x frame ph + d*i - pad: activation, zero borders and the
         # de-interleave in ONE launch (st5_lrelu_pad; slope 1 = plain copy)
         buf = torch.empty((B, n_in, Cin), dtype=torch.bfloat16, device=x.device)
-        K.lrelu_pad(x, buf, d, ph, pad, pre_act_slope if pre_act_slope is not None else 1.0)
+        _stage(x, buf, d, ph, pad, pre_act_slope if pre_act_slope is not None else 1.0, lengths, len_mult)
         kw = dict(M=n_out, N=Cout, K=k * Cin, a_ld=Cin, b_ld=conv.ld, c_ld=d * Cout, nb1=B, nb2=1, a_bs=(n_in * Cin, 0),
                   b_bs=(0, 0), c_bs=(T * Cout, 0), bias=conv.bias, act=act)
         if residual is not None:
@@ -93,11 +109,11 @@ class _ConvT:
             self.phases.append((min(ds), len(ds), w, ld))
 
 
-def _conv_transpose(x, ct, pre_act_slope=None):
+def _conv_transpose(x, ct, pre_act_slope=None, lengths=None, len_mult=1):
     B, T, Cin = x.shape
     fr = ct.taps - 1
     buf = torch.empty((B, T + 2 * fr, Cin), dtype=torch.bfloat16, device=x.device)
-    K.lrelu_pad(x.contiguous(), buf, 1, 0, fr, pre_act_slope if pre_act_slope is not None else 1.0)
+    _stage(x.contiguous(), buf, 1, 0, fr, pre_act_slope if pre_act_slope is not None else 1.0, lengths, len_mult)
     y = torch.empty((B, T * ct.u, ct.cout), dtype=torch.bfloat16, device=x.device)
     Tp = T + 2 * fr
     for r, (d0, nt, w, ld) in enumerate(ct.phases):
@@ -107,15 +123,46 @@ def _conv_transpose(x, ct, pre_act_slope=None):
     return y
 
 
+def _fold(g, v):
+    """torch.nn.utils.weight_norm(dim=0): weight = v * (g / ||v||), the norm over every dimension but the first."""
+    norm = v.reshape(v.size(0), -1).norm(dim=1).view(-1, *([1] * (v.dim() - 1)))
+    return v * (g / norm)
+
+
+def plain_state_dict(state_dict):
+    """A generator state dict in the key names this module reads (`conv_pre`, `ups.{i}`, `resblocks.{r}.convs1.{j}`,
+    `conv_post`, `mean`, `scale`, plain `.weight` / `.bias`), from any of the names the same tensors are published under:
+    fairseq / SpeechUT (`ups.{i}`), HuggingFace SpeechT5HifiGan (`upsampler.{i}`), with weight norm either folded or as
+    `weight_g` / `weight_v` pairs."""
+    out = {}
+    for k, v in state_dict.items():
+        if k.endswith(".weight_v"):
+            continue
+        if k.endswith(".weight_g"):
+            base = k[:-len("_g")]
+            k, v = base, _fold(v, state_dict[base + "_v"])
+        if k.startswith("upsampler."):
+            k = "ups." + k[len("upsampler."):]
+        out[k] = v
+    return out
+
+
 class HifiGanGenerator:
-    """Inference-only generator built from a state dict with the oracle's / reference's key names (weight norm folded:
-    `conv_pre.weight`, `ups.{i}.weight`, `resblocks.{r}.convs1.{j}.weight`, ..., `conv_post.weight`, `mean`, `scale`)."""
+    """Inference-only generator built from a state dict (key names: see plain_state_dict; a state dict without `mean` /
+    `scale` normalises with 0 / 1). cfg: the fields of HIFIGAN_CFG, named as in SpeechT5HifiGanConfig, plus
+    `leaky_relu_slope`; other keys are ignored, so a HuggingFace config.json dict can be passed as it is."""
 
     def __init__(self, state_dict, cfg=None, device="cuda"):
-        cfg = dict(HIFIGAN_CFG, **(cfg or {}))
+        cfg = dict(cfg or {})
+        self.lrelu_slope = float(cfg.get("leaky_relu_slope", LRELU_SLOPE))
+        cfg = dict(HIFIGAN_CFG, **{k: v for k, v in cfg.items() if k in HIFIGAN_CFG})
         self.cfg = cfg
-        sd = {k: v.to(device) for k, v in state_dict.items()}
-        self.mean, self.scale = sd["mean"].float(), sd["scale"].float()
+        sd = {k: v.to(device) for k, v in plain_state_dict(state_dict).items()}
+        C0 = cfg["model_in_dim"]
+        self.mean = sd["mean"].float() if "mean" in sd else torch.zeros(C0, device=device)
+        self.scale = sd["scale"].float() if "scale" in sd else torch.ones(C0, device=device)
+        self.device = self.mean.device
+        self.hop = math.prod(cfg["upsample_rates"])  # waveform samples per mel frame
         self.conv_pre = _Conv(sd["conv_pre.weight"], sd["conv_pre.bias"])
         self.ups = [_ConvT(sd[f"ups.{i}.weight"], sd[f"ups.{i}.bias"], u, (k - u) // 2)
                     for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"]))]
@@ -131,11 +178,17 @@ class HifiGanGenerator:
                 self.resblocks.append((c1, c2))
                 r += 1
         self.conv_post = _Conv(sd["conv_post.weight"], sd["conv_post.bias"])
+        self._graphs = {}  # (B, T_bucket, normalize_before, device) -> _VocodeGraph
 
     @torch.no_grad()
     def __call__(self, spectrogram, normalize_before=True):
         """spectrogram [B, T, 80] fp32 log-mel -> waveform [B, T * prod(upsample_rates)] fp32."""
         K._require_cuda(spectrogram)
+        return self._forward(spectrogram, normalize_before)
+
+    def _forward(self, spectrogram, normalize_before, lengths=None):
+        """The generator on [B, T, model_in_dim]; lengths (int32 [B] device tensor, mel frames): row b is computed as
+        if the input ended at its length (output samples past lengths[b] * prod(upsample_rates) are not meaningful)."""
         x = spectrogram.float()
         if normalize_before:
             x = (x - self.mean) / self.scale
@@ -145,18 +198,98 @@ class HifiGanGenerator:
         xb[..., :C0] = x.to(torch.bfloat16)
         if ld0 != C0:
             raise NotImplementedError("model_in_dim must be a multiple of 8 (80 in the release)")
-        x = _conv_same(xb, self.conv_pre)
+        x = _conv_same(xb, self.conv_pre, lengths=lengths)
+        mult = 1  # frames of x per mel frame
         for i, up in enumerate(self.ups):
-            x = _conv_transpose(x, up, pre_act_slope=LRELU_SLOPE)
+            x = _conv_transpose(x, up, pre_act_slope=self.lrelu_slope, lengths=lengths, len_mult=mult)
+            mult *= up.u
             xs = None
             for j in range(self.num_kernels):
                 c1s, c2s = self.resblocks[i * self.num_kernels + j]
                 h = x
                 for c1, c2 in zip(c1s, c2s):
-                    t = _conv_same(h, c1, pre_act_slope=LRELU_SLOPE)
-                    h = _conv_same(t, c2, residual=h, pre_act_slope=LRELU_SLOPE)
+                    t = _conv_same(h, c1, pre_act_slope=self.lrelu_slope, lengths=lengths, len_mult=mult)
+                    h = _conv_same(t, c2, residual=h, pre_act_slope=self.lrelu_slope, lengths=lengths, len_mult=mult)
                 xs = h.float() if xs is None else xs + h.float()
             x = (xs / self.num_kernels).to(torch.bfloat16)
         y = torch.empty((x.shape[0], x.shape[1], 1), dtype=torch.float32, device=x.device)
-        _conv_same(x, self.conv_post, out=y, act="tanh", pre_act_slope=0.01)  # (default slope here, reference :165)
+        # (default slope here, reference :165)
+        _conv_same(x, self.conv_post, out=y, act="tanh", pre_act_slope=0.01, lengths=lengths, len_mult=mult)
         return y[..., 0]
+
+    def _check_mels(self, mels):
+        """Host-side validation of vocode's input (raises ValueError; nothing is launched)."""
+        if not isinstance(mels, (list, tuple)) or len(mels) == 0:
+            raise ValueError("vocode takes a non-empty list of [L, model_in_dim] mel tensors")
+        C0 = self.cfg["model_in_dim"]
+        for b, m in enumerate(mels):
+            if not torch.is_tensor(m) or m.dim() != 2 or m.shape[1] != C0:
+                raise ValueError(f"mel {b}: expected a [L, {C0}] tensor, got "
+                                 f"{tuple(m.shape) if torch.is_tensor(m) else type(m).__name__}")
+            if m.shape[0] < 1:
+                raise ValueError(f"mel {b}: empty (L = 0)")
+            if m.dtype != torch.float32:
+                raise ValueError(f"mel {b}: dtype {m.dtype}, expected torch.float32")
+            if m.device != self.device:
+                raise ValueError(f"mel {b}: on {m.device}, the vocoder is on {self.device}")
+
+    @torch.no_grad()
+    def vocode(self, mels, normalize_before=True):
+        """Vocode utterances of different lengths in one CUDA-graph replay: mels = list of [L_b, model_in_dim] fp32
+        device tensors -> list of [L_b * prod(upsample_rates)] fp32 waveforms, each bitwise equal to
+        self(mels[b][None], normalize_before)[0]. The batch is padded to a bucket of 64 frames; one graph is captured
+        per (B, bucket, normalize_before, device) and kept on the generator."""
+        self._check_mels(mels)
+        T_b = max(64, (max(m.shape[0] for m in mels) + 63) // 64 * 64)
+        key = (len(mels), T_b, bool(normalize_before), str(self.device))
+        vg = self._graphs.get(key)
+        if vg is None:
+            vg = self._graphs[key] = _VocodeGraph(self, len(mels), T_b, bool(normalize_before))
+        return vg.run(mels)
+
+
+class _VocodeGraph:
+    """One generator pass over B utterances padded to T_bucket frames, reading the static buffers `mel` [B, T_bucket,
+    model_in_dim] and `lengths` (int32 [B]): captured once, replayed for every batch of the same size and bucket. Frames
+    of `mel` past an utterance's length are never read. capture=False runs the same body eagerly."""
+
+    def __init__(self, gen, B, T_bucket, normalize_before, capture=True):
+        self.gen, self.B, self.T, self.normalize_before, self.capture = gen, B, T_bucket, normalize_before, capture
+        dev = gen.device
+        self.mel = torch.zeros((B, T_bucket, gen.cfg["model_in_dim"]), dtype=torch.float32, device=dev)
+        self.lengths = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.graph, self.out, self.launches = None, None, 0
+
+    def _body(self):
+        n0 = K.LAUNCHES
+        out = self.gen._forward(self.mel, self.normalize_before, self.lengths)
+        self.launches = K.LAUNCHES - n0  # library kernels per pass (a replay does not go through kernels.py)
+        return out
+
+    def _capture(self):
+        dev = self.gen.device
+        stream = torch.cuda.Stream(device=dev)
+        stream.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(stream):
+            self._body()  # warm-up outside the capture (first-call setup of the library and the allocator)
+            stream.synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=stream):
+                self.out = self._body()
+        torch.cuda.current_stream(dev).wait_stream(stream)
+        self.graph = g
+
+    def run(self, mels):
+        lens = [m.shape[0] for m in mels]
+        assert len(mels) == self.B and max(lens) <= self.T
+        for b, m in enumerate(mels):
+            self.mel[b, :lens[b]].copy_(m)
+        self.lengths.copy_(torch.tensor(lens, dtype=torch.int32))
+        if not self.capture:
+            self.out = self._body()
+        else:
+            if self.graph is None:
+                self._capture()
+            self.graph.replay()
+        hop = self.gen.hop
+        return [self.out[b, :L * hop].clone() for b, L in enumerate(lens)]
