@@ -96,12 +96,14 @@ class ConvFeatureExtractionModel(nn.Module):
         x = x.unsqueeze(1)
         for blk in self.conv_layers:
             for m in blk:
-                # Fp32LayerNorm (between TransposeLast) / Fp32GroupNorm: statistics in (at least) fp32
+                # Fp32LayerNorm (between TransposeLast) / Fp32GroupNorm: input AND affine parameters in (at least) fp32
                 hi = x if x.dtype in (torch.float32, torch.float64) else x.float()
+                w, b = (None if v is None else v.to(hi.dtype)
+                        for v in (getattr(m, "weight", None), getattr(m, "bias", None)))
                 if isinstance(m, nn.LayerNorm):
-                    x = m(hi.transpose(1, 2)).transpose(1, 2).type_as(x)
+                    x = F.layer_norm(hi.transpose(1, 2), m.normalized_shape, w, b, m.eps).transpose(1, 2).type_as(x)
                 elif isinstance(m, nn.GroupNorm):
-                    x = m(hi).type_as(x)
+                    x = F.group_norm(hi, m.num_groups, w, b, m.eps).type_as(x)
                 else:
                     x = m(x)
         return x
