@@ -117,6 +117,13 @@ int st5_ln_fwd(const void* x, const void* residual, const float* gamma, const fl
 int st5_ln_fwd_stream(const void* x, const void* residual, const float* residual_f32, const float* gamma,
                       const float* beta, void* y, float* y_f32, void* s_out, float* mean, float* rstd, int dtype,
                       int64_t rows, int64_t C, float eps, float drop_p, uint64_t seed, uint64_t offset, void* stream);
+/* Forward only, for rows wider than st5_ln_fwd takes (the 1280-wide pre-LN layers of transformer_lm_t5,
+ * speecht5/models/t5_transformer_lm.py:16-25): y = LN(x + residual) * gamma + beta with the arithmetic of
+ * st5_ln_fwd (fp32 statistics, two-pass variance) for 8 <= C <= 2048, C % 8 == 0, no dropout and no saved sum. residual,
+ * mean and rstd may be NULL; x, residual, y, gamma and beta must be 16-byte aligned. Anything else returns -2 before any
+ * launch. st5_ln_fwd, st5_ln_fwd_stream and st5_ln_bwd keep C <= 1024: rows this wide have no backward. */
+int st5_ln_fwd_wide(const void* x, const void* residual, const float* gamma, const float* beta, void* y, float* mean,
+                    float* rstd, int dtype, int64_t rows, int64_t C, float eps, void* stream);
 /* ds = LN backward wrt s; dx = dropout-backward(ds) (may alias / be NULL when drop_p == 0 and caller reuses ds);
  * dgamma/dbeta are accumulated (+=) in fp32. `dxsum` (may be NULL; fp32 [C], accumulated +=) receives the column sums
  * of dx (of ds when dx is NULL): in the post-LN tail y = LN(residual + dropout(W a + b)) that is the gradient of b, so
@@ -236,6 +243,18 @@ typedef struct st5_attn_lineage_args {
   int32_t kv_div;
 } st5_attn_lineage_args;
 int st5_attn_lineage_fwd(const st5_attn_lineage_args* args, void* stream);
+
+/* The two one-row attentions above for a head width `head_dim` of 64 or 80 (transformer_lm_t5, 1280 channels in 16
+ * heads: speecht5/models/t5_transformer_lm.py:16-25): every "64" of their index formulas reads head_dim, and the
+ * argument structs, the split-KV contract and the error codes are theirs. head_dim 64 launches exactly the kernels of
+ * st5_attn_decode_fwd / st5_attn_lineage_fwd (bit-identical results); head_dim 80 launches their 80-wide counterparts:
+ * splits of 64 keys, key j in split j / 64 at a fixed position, masked keys never loaded and adding an exact zero, so a
+ * row's result is bit-identical at any B and any key span that holds its valid keys; a row whose keys are all masked
+ * gives zeros. Any other head_dim returns -2 before any launch (and st5_attn_decode_hd_ws_floats returns -2 for it);
+ * ws: st5_attn_decode_hd_ws_floats(B, H, Tk, probs != NULL, head_dim) floats (none for Tk <= 64). */
+int64_t st5_attn_decode_hd_ws_floats(int32_t B, int32_t H, int32_t Tk, int32_t with_probs, int32_t head_dim);
+int st5_attn_decode_hd_fwd(const st5_attn_decode_args* args, int32_t head_dim, void* stream);
+int st5_attn_lineage_hd_fwd(const st5_attn_lineage_args* args, int32_t head_dim, void* stream);
 
 /* Beam search candidate selection (sequence_generator.py:430-454 with fairseq/search.py:117-144, BeamSearch.step) for B
  * sentences of K beams (1 <= K <= 16, rows r = s * K + k), vocabulary V (1 < V <= 32768). Per row, fp32:

@@ -74,6 +74,7 @@ _PROTOS = {
     "st5_ln_fwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _f, _f, _u64, _u64, _vp]),
     "st5_ln_fwd_stream": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _f, _f, _u64,
                                     _u64, _vp]),
+    "st5_ln_fwd_wide": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _f, _vp]),
     "st5_ln_bwd_blocks": (C.c_int64, [_i64]),
     "st5_ln_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _f, _u64, _u64, _vp]),
     "st5_lrelu_pad": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _f, _vp]),
@@ -86,6 +87,9 @@ _PROTOS = {
     "st5_attn_decode_ws_floats": (C.c_int64, [_i32, _i32, _i32, _i32]),
     "st5_attn_decode_fwd": (C.c_int, [C.POINTER(AttnDecodeArgs), _vp]),
     "st5_attn_lineage_fwd": (C.c_int, [C.POINTER(AttnLineageArgs), _vp]),
+    "st5_attn_decode_hd_ws_floats": (C.c_int64, [_i32, _i32, _i32, _i32, _i32]),
+    "st5_attn_decode_hd_fwd": (C.c_int, [C.POINTER(AttnDecodeArgs), _i32, _vp]),
+    "st5_attn_lineage_hd_fwd": (C.c_int, [C.POINTER(AttnLineageArgs), _i32, _vp]),
     "st5_beam_topk_ws_floats": (C.c_int64, [_i32, _i32]),
     "st5_beam_topk": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _f, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                 _vp]),

@@ -95,6 +95,11 @@ int st5_ln_fwd_stream(const void* x, const void* residual, const float* residual
                                  eps, drop_p, seed, offset, (cudaStream_t)stream),
                    "st5_ln_fwd_stream");
 }
+int st5_ln_fwd_wide(const void* x, const void* residual, const float* gamma, const float* beta, void* y, float* mean,
+                    float* rstd, int dtype, int64_t rows, int64_t C, float eps, void* stream) {
+  return set_error(ln_fwd_wide_launch(x, residual, gamma, beta, y, mean, rstd, dtype, rows, C, eps, (cudaStream_t)stream),
+                   "st5_ln_fwd_wide");
+}
 int64_t st5_ln_bwd_blocks(int64_t rows) { return ln_bwd_blocks(rows); }
 int st5_ln_bwd(const void* dy, const void* s, const float* mean, const float* rstd, const float* gamma, void* ds,
                void* dx, float* dgamma, float* dbeta, float* dxsum, int dtype, int64_t rows, int64_t C, float drop_p,
@@ -144,6 +149,15 @@ int st5_attn_decode_fwd(const st5_attn_decode_args* a, void* stream) {
 }
 int st5_attn_lineage_fwd(const st5_attn_lineage_args* a, void* stream) {
   return set_error(attn_lineage_launch(*a, (cudaStream_t)stream), "st5_attn_lineage_fwd");
+}
+int64_t st5_attn_decode_hd_ws_floats(int32_t B, int32_t H, int32_t Tk, int32_t with_probs, int32_t head_dim) {
+  return attn_decode_hd_ws_floats(B, H, Tk, with_probs, head_dim);
+}
+int st5_attn_decode_hd_fwd(const st5_attn_decode_args* a, int32_t head_dim, void* stream) {
+  return set_error(attn_decode_hd_launch(*a, head_dim, (cudaStream_t)stream), "st5_attn_decode_hd_fwd");
+}
+int st5_attn_lineage_hd_fwd(const st5_attn_lineage_args* a, int32_t head_dim, void* stream) {
+  return set_error(attn_lineage_hd_launch(*a, head_dim, (cudaStream_t)stream), "st5_attn_lineage_hd_fwd");
 }
 
 int64_t st5_beam_topk_ws_floats(int32_t B, int32_t K) { return beam_topk_ws_floats(B, K); }

@@ -131,6 +131,8 @@ int posenc_bwd_launch(const void* dy, const int64_t* tokens, int64_t padding_idx
 int ln_fwd_launch(const void* x, const void* residual, const float* residual_f32, const float* gamma, const float* beta,
                   void* y, float* y_f32, void* s_out, float* mean, float* rstd, int dtype, int64_t rows, int64_t C,
                   float eps, float drop_p, uint64_t seed, uint64_t offset, cudaStream_t s);
+int ln_fwd_wide_launch(const void* x, const void* residual, const float* gamma, const float* beta, void* y, float* mean,
+                       float* rstd, int dtype, int64_t rows, int64_t C, float eps, cudaStream_t s);
 int64_t ln_bwd_blocks(int64_t rows);
 int ln_bwd_launch(const void* dy, const void* s_in, const float* mean, const float* rstd, const float* gamma, void* ds,
                   void* dx, float* dgamma, float* dbeta, float* dxsum, int dtype, int64_t rows, int64_t C,
@@ -148,6 +150,9 @@ int attn_bwd_launch(const st5_attn_args& a, cudaStream_t s);
 int64_t attn_decode_ws_floats(int B, int H, int Tk, int with_probs);
 int attn_decode_launch(const st5_attn_decode_args& a, cudaStream_t s);
 int attn_lineage_launch(const st5_attn_lineage_args& a, cudaStream_t s);
+int64_t attn_decode_hd_ws_floats(int B, int H, int Tk, int with_probs, int head_dim);
+int attn_decode_hd_launch(const st5_attn_decode_args& a, int head_dim, cudaStream_t s);
+int attn_lineage_hd_launch(const st5_attn_lineage_args& a, int head_dim, cudaStream_t s);
 int64_t beam_topk_ws_floats(int B, int K);
 int beam_topk_launch(const void* logits, int64_t ld, int dtype, int B, int K, int V, const float* cum,
                      const float* mask, float inv_temp, int eos, const int64_t* t, const int64_t* min_len,

@@ -117,6 +117,87 @@ int ln_fwd_launch(const void* x, const void* residual, const float* residual_f32
   return (int)cudaGetLastError();
 }
 
+// Forward only, for rows past LN_MAX_CHUNKS (the pre-LN layers of a 1280-wide language model): the arithmetic of
+// ln_fwd_kernel -- each lane's chunks summed in order, warp sums, two-pass variance, rsqrtf -- with eight chunks per lane
+// (C <= 8 * 32 * 8 = 2048) and neither dropout nor a saved sum, so it adds no backward state to keep.
+constexpr int LN_WIDE_CHUNKS = 8;
+
+template <typename T>
+__global__ void __launch_bounds__(LN_WARPS * 32)
+    ln_fwd_wide_kernel(const T* __restrict__ x, const T* __restrict__ residual, const float* __restrict__ gamma,
+                       const float* __restrict__ beta, T* __restrict__ y, float* __restrict__ mean,
+                       float* __restrict__ rstd, int64_t rows, int C, float eps) {
+  pdl_sync();
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * LN_WARPS + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const int nchunks = C >> 3;
+  float v[LN_WIDE_CHUNKS][8];
+  float sum = 0.f;
+#pragma unroll
+  for (int k = 0; k < LN_WIDE_CHUNKS; ++k) {
+    const int ch = k * 32 + lane;
+    if (ch < nchunks) {
+      const int64_t e0 = row * C + ch * 8;
+      load8<T>(x + e0, v[k]);
+      if (residual != nullptr) {
+        float r[8];
+        load8<T>(residual + e0, r);
+#pragma unroll
+        for (int t = 0; t < 8; ++t) v[k][t] += r[t];
+      }
+#pragma unroll
+      for (int t = 0; t < 8; ++t) sum += v[k][t];
+    }
+  }
+  sum = warp_sum(sum);
+  const float mu = sum / (float)C;
+  float sq = 0.f;
+#pragma unroll
+  for (int k = 0; k < LN_WIDE_CHUNKS; ++k) {
+    if (k * 32 + lane < nchunks) {
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+        const float d = v[k][t] - mu;
+        sq += d * d;
+      }
+    }
+  }
+  sq = warp_sum(sq);
+  const float rs = rsqrtf(sq / (float)C + eps);
+  if (lane == 0) {
+    if (mean != nullptr) mean[row] = mu;
+    if (rstd != nullptr) rstd[row] = rs;
+  }
+#pragma unroll
+  for (int k = 0; k < LN_WIDE_CHUNKS; ++k) {
+    const int ch = k * 32 + lane;
+    if (ch < nchunks) {
+      float g[8], b[8], o[8];
+      load8<float>(gamma + ch * 8, g);
+      load8<float>(beta + ch * 8, b);
+#pragma unroll
+      for (int t = 0; t < 8; ++t) o[t] = (v[k][t] - mu) * rs * g[t] + b[t];
+      store8<T>(y + row * C + ch * 8, o);
+    }
+  }
+}
+
+int ln_fwd_wide_launch(const void* x, const void* residual, const float* gamma, const float* beta, void* y, float* mean,
+                       float* rstd, int dtype, int64_t rows, int64_t C, float eps, cudaStream_t s) {
+  if (rows == 0) return 0;
+  if (C > 8 * 32 * LN_WIDE_CHUNKS || C < 8 || (C & 7) || rows < 0) return -2;
+  if (!ln_aligned({x, residual, gamma, beta, y})) return -2;
+  const unsigned grid = (unsigned)((rows + LN_WARPS - 1) / LN_WARPS);
+  if (dtype == ST5_F32)
+    launch_pdl(ln_fwd_wide_kernel<float>, dim3(grid), dim3(LN_WARPS * 32), 0, s, (const float*)x,
+               (const float*)residual, gamma, beta, (float*)y, mean, rstd, rows, (int)C, eps);
+  else
+    launch_pdl(ln_fwd_wide_kernel<__nv_bfloat16>, dim3(grid), dim3(LN_WARPS * 32), 0, s, (const __nv_bfloat16*)x,
+               (const __nv_bfloat16*)residual, gamma, beta, (__nv_bfloat16*)y, mean, rstd, rows, (int)C, eps);
+  return (int)cudaGetLastError();
+}
+
 // number of floats of scratch the caller provides (kept for ABI stability; the reduction now uses fp32 atomics)
 int64_t ln_bwd_blocks(int64_t rows) { (void)rows; return 1; }
 

@@ -133,6 +133,16 @@ def ln_fwd(x, residual, gamma, beta, y, s_out, mean, rstd, eps, drop_p=0.0, seed
     _count(1)
 
 
+def ln_fwd_wide(x, residual, gamma, beta, y, mean=None, rstd=None, eps=1e-5):
+    """st5_ln_fwd_wide: y = LayerNorm(x + residual) for rows of 8 <= C <= 2048 channels, forward only (no dropout)."""
+    _require_cuda(x, residual, gamma, beta, y, mean, rstd)
+    Cc = x.shape[-1]
+    rows = x.numel() // Cc
+    _lib.check(_lib.load().st5_ln_fwd_wide(_ptr(x), _ptr(residual), _ptr(gamma), _ptr(beta), _ptr(y), _ptr(mean),
+                                           _ptr(rstd), dtype_id(x), rows, Cc, eps, _stream()), "st5_ln_fwd_wide")
+    _count(1)
+
+
 def ln_bwd(dy, s, mean, rstd, gamma, ds, dx, dgamma, dbeta, drop_p=0.0, seed=0, offset=0, dxsum=None):
     """dxsum (optional, fp32 [C], accumulated): column sums of dx = the bias gradient of the projection that fed x."""
     Cc = dy.shape[-1]
@@ -209,6 +219,20 @@ def attn_fwd(a):
     _count(1)
 
 
+def _decode_fields(d, B, q, k, v, out, H, scale, key_pad, probs, ws):
+    """Fill an AttnDecodeArgs from strided views: q [B, 1, H*hd], k / v [*, Tk, H*hd], out [B, 1, H*hd]."""
+    d.B, d.H, d.Tk, d.dtype = B, H, k.shape[1], dtype_id(out)
+    d.q, d.q_bs = q.data_ptr(), q.stride(0)
+    d.k, d.k_ld, d.k_bs = k.data_ptr(), k.stride(1), k.stride(0)
+    d.v, d.v_ld, d.v_bs = v.data_ptr(), v.stride(1), v.stride(0)
+    d.key_pad, d.out, d.o_bs, d.probs = _ptr(key_pad), out.data_ptr(), out.stride(0), _ptr(probs)
+    d.scale, d.ws = scale, _ptr(ws)
+
+
+def _decode_ws(nws, out):
+    return torch.empty(nws, dtype=torch.float32, device=out.device) if nws > 0 else None
+
+
 def attn_decode_fwd(q, k, v, out, *, H, scale, key_pad=None, probs=None):
     """st5_attn_decode_fwd (include/speecht5_b200.h): one query row per (utterance, head). q [B, 1, H*64] and
     k / v [B, Tk, H*64] are strided views (e.g. column blocks of a fused projection buffer), out [B, 1, H*64];
@@ -219,14 +243,8 @@ def attn_decode_fwd(q, k, v, out, *, H, scale, key_pad=None, probs=None):
     assert probs is None or (probs.dtype == torch.float32 and probs.is_contiguous() and probs.numel() == B * H * Tk)
     lib = _lib.load()
     nws = lib.st5_attn_decode_ws_floats(B, H, Tk, int(probs is not None))
-    ws = torch.empty(nws, dtype=torch.float32, device=out.device) if nws > 0 else None
     a = _lib.AttnDecodeArgs()
-    a.B, a.H, a.Tk, a.dtype = B, H, Tk, dtype_id(out)
-    a.q, a.q_bs = q.data_ptr(), q.stride(0)
-    a.k, a.k_ld, a.k_bs = k.data_ptr(), k.stride(1), k.stride(0)
-    a.v, a.v_ld, a.v_bs = v.data_ptr(), v.stride(1), v.stride(0)
-    a.key_pad, a.out, a.o_bs, a.probs = _ptr(key_pad), out.data_ptr(), out.stride(0), _ptr(probs)
-    a.scale, a.ws = scale, _ptr(ws)
+    _decode_fields(a, B, q, k, v, out, H, scale, key_pad, probs, _decode_ws(nws, out))
     _lib.check(lib.st5_attn_decode_fwd(C.byref(a), _stream()), "st5_attn_decode_fwd")
     _count(1 if nws == 0 else 2)
 
@@ -240,17 +258,44 @@ def attn_lineage_fwd(q, k, v, out, *, H, scale, key_pad=None, kv_rows=None, kv_d
     assert kv_rows is None or (kv_rows.dtype == torch.int32 and kv_rows.stride(1) == 1 and kv_rows.shape[0] == B)
     lib = _lib.load()
     nws = lib.st5_attn_decode_ws_floats(B, H, Tk, 0)
-    ws = torch.empty(nws, dtype=torch.float32, device=out.device) if nws > 0 else None
     a = _lib.AttnLineageArgs()
-    d = a.base
-    d.B, d.H, d.Tk, d.dtype = B, H, Tk, dtype_id(out)
-    d.q, d.q_bs = q.data_ptr(), q.stride(0)
-    d.k, d.k_ld, d.k_bs = k.data_ptr(), k.stride(1), k.stride(0)
-    d.v, d.v_ld, d.v_bs = v.data_ptr(), v.stride(1), v.stride(0)
-    d.key_pad, d.out, d.o_bs, d.probs = _ptr(key_pad), out.data_ptr(), out.stride(0), None
-    d.scale, d.ws = scale, _ptr(ws)
+    _decode_fields(a.base, B, q, k, v, out, H, scale, key_pad, None, _decode_ws(nws, out))
     a.kv_rows, a.kv_rows_ld, a.kv_div = _ptr(kv_rows), (kv_rows.stride(0) if kv_rows is not None else 0), kv_div
     _lib.check(lib.st5_attn_lineage_fwd(C.byref(a), _stream()), "st5_attn_lineage_fwd")
+    _count(1 if nws == 0 else 2)
+
+
+def attn_decode_hd_fwd(q, k, v, out, *, H, head_dim, scale, key_pad=None, probs=None):
+    """st5_attn_decode_hd_fwd: attn_decode_fwd for heads of `head_dim` (64 or 80) channels, q / out [B, 1, H*head_dim],
+    k / v [B, Tk, H*head_dim]."""
+    _require_cuda(q, k, v, out, key_pad, probs)
+    assert q.dtype == k.dtype == v.dtype == out.dtype and k.stride(2) == 1 and v.stride(2) == 1
+    B, Tk = k.shape[0], k.shape[1]
+    assert probs is None or (probs.dtype == torch.float32 and probs.is_contiguous() and probs.numel() == B * H * Tk)
+    lib = _lib.load()
+    nws = lib.st5_attn_decode_hd_ws_floats(B, H, Tk, int(probs is not None), head_dim)
+    if nws < 0:
+        raise ValueError(f"one-row attention over heads of {head_dim} channels: 64 and 80 are built")
+    a = _lib.AttnDecodeArgs()
+    _decode_fields(a, B, q, k, v, out, H, scale, key_pad, probs, _decode_ws(nws, out))
+    _lib.check(lib.st5_attn_decode_hd_fwd(C.byref(a), head_dim, _stream()), "st5_attn_decode_hd_fwd")
+    _count(1 if nws == 0 else 2)
+
+
+def attn_lineage_hd_fwd(q, k, v, out, *, H, head_dim, scale, key_pad=None, kv_rows=None, kv_div=1):
+    """st5_attn_lineage_hd_fwd: attn_lineage_fwd for heads of `head_dim` (64 or 80) channels."""
+    _require_cuda(q, k, v, out, key_pad, kv_rows)
+    assert q.dtype == k.dtype == v.dtype == out.dtype and k.stride(2) == 1 and v.stride(2) == 1
+    B, Tk = q.shape[0], k.shape[1]
+    assert kv_rows is None or (kv_rows.dtype == torch.int32 and kv_rows.stride(1) == 1 and kv_rows.shape[0] == B)
+    lib = _lib.load()
+    nws = lib.st5_attn_decode_hd_ws_floats(B, H, Tk, 0, head_dim)
+    if nws < 0:
+        raise ValueError(f"one-row attention over heads of {head_dim} channels: 64 and 80 are built")
+    a = _lib.AttnLineageArgs()
+    _decode_fields(a.base, B, q, k, v, out, H, scale, key_pad, None, _decode_ws(nws, out))
+    a.kv_rows, a.kv_rows_ld, a.kv_div = _ptr(kv_rows), (kv_rows.stride(0) if kv_rows is not None else 0), kv_div
+    _lib.check(lib.st5_attn_lineage_hd_fwd(C.byref(a), head_dim, _stream()), "st5_attn_lineage_hd_fwd")
     _count(1 if nws == 0 else 2)
 
 

@@ -2,9 +2,11 @@
 fairseq's `transformer_lm` (fairseq/models/transformer_lm.py:200-362 with the TransformerDecoder of
 fairseq/models/transformer.py:637-986, no encoder attention) on this package's kernels.
 
-Built configuration: pre-LN decoder layers (base_lm_architecture forces decoder_normalize_before), sinusoidal or learned
-positions at padding_idx + 1 + i, embed_scale = sqrt(C) unless no_scale_embedding, an optional final LayerNorm
-(no_decoder_final_norm), an output projection tied to the embedding or not, relu or gelu. Adaptive input or softmax,
+Built configuration: heads of 64 or 80 channels (80: SpeechT5's own `transformer_lm_t5`, 1280 channels in 16 heads,
+whose preset applies when the arguments name that arch), rows up to 2048 channels, pre-LN decoder layers
+(base_lm_architecture forces decoder_normalize_before), sinusoidal or learned positions at padding_idx + 1 + i,
+embed_scale = sqrt(C) unless no_scale_embedding, an optional final LayerNorm (no_decoder_final_norm), an output
+projection tied to the embedding or not, relu or gelu. Adaptive input or softmax,
 character embeddings, layernorm_embedding, project_in / project_out dimensions, cross_self_attention and quant noise
 raise NotImplementedError when the model is built.
 
@@ -22,6 +24,67 @@ from .models.modules.transformer import TransformerDecoderLayer
 
 # fairseq keeps these buffers in a transformer_lm state dict; they carry no weights
 _BUFFERS = ("decoder.version", "decoder.embed_positions._float_tensor")
+HEAD_DIMS = (64, 80)  # the one-row attention's head widths (80: transformer_lm_t5, 1280 channels in 16 heads)
+MAX_DIM = 2048        # the widest LayerNorm row (st5_ln_fwd_wide)
+
+# fairseq's base_lm_architecture (fairseq/models/transformer_lm.py:296-359): an option the arguments lack takes this value
+_BASE_LM_DEFAULTS = dict(
+    dropout=0.1, attention_dropout=0.0, decoder_embed_dim=512, decoder_ffn_embed_dim=2048, decoder_layers=6,
+    decoder_attention_heads=8, adaptive_softmax_cutoff=None, adaptive_softmax_dropout=0, adaptive_softmax_factor=4,
+    decoder_learned_pos=False, activation_fn="relu", decoder_layerdrop=0, decoder_layers_to_keep=None, quant_noise_pq=0,
+    quant_noise_pq_block_size=8, quant_noise_scalar=0, base_layers=0, base_sublayers=1, base_shuffle=False,
+    add_bos_token=False, no_token_positional_embeddings=False, share_decoder_input_output_embed=False,
+    character_embeddings=False)
+_BASE_LM_DEFAULTS_TAIL = dict(no_decoder_final_norm=False, adaptive_input=False, adaptive_input_factor=4,
+                              adaptive_input_cutoff=None, tie_adaptive_weights=False, tie_adaptive_proj=False,
+                              no_scale_embedding=False, layernorm_embedding=False, checkpoint_activations=False,
+                              offload_activations=False)
+# SpeechT5's own LM (speecht5/models/t5_transformer_lm.py: arch transformer_lm_t5), applied before the base defaults
+_T5_LM_DEFAULTS = dict(decoder_embed_dim=1280, decoder_ffn_embed_dim=6144, decoder_layers=20, decoder_attention_heads=16,
+                       dropout=0.1, attention_dropout=0.1, activation_fn="gelu")
+
+
+def _fill(args, defaults):
+    for k, v in defaults.items():
+        if not hasattr(args, k):
+            setattr(args, k, v)
+
+
+def base_lm_architecture(args):
+    """Fill `args` in place as fairseq's base_lm_architecture does: options it lacks take their defaults (an option set
+    to None stays None), decoder_input_dim / decoder_output_dim follow decoder_embed_dim, the layers are pre-LN, and the
+    compatibility rules for old checkpoints (no_tie_adaptive_proj, decoder_final_norm) apply."""
+    if hasattr(args, "no_tie_adaptive_proj"):
+        args.no_decoder_final_norm = True
+        if args.no_tie_adaptive_proj is False:
+            args.tie_adaptive_proj = True
+    if hasattr(args, "decoder_final_norm"):
+        args.no_decoder_final_norm = not args.decoder_final_norm
+    _fill(args, _BASE_LM_DEFAULTS)
+    _fill(args, dict(decoder_output_dim=args.decoder_embed_dim, decoder_input_dim=args.decoder_embed_dim))
+    args.decoder_normalize_before = True
+    _fill(args, _BASE_LM_DEFAULTS_TAIL)
+    if args.offload_activations:
+        args.checkpoint_activations = True
+    return args
+
+
+def transformer_lm_t5(args):
+    """The `transformer_lm_t5` preset, in place: 20 layers of 1280 channels, 16 heads of 80, FFN 6144, GELU, dropout
+    0.1 for options `args` lacks, then base_lm_architecture."""
+    _fill(args, _T5_LM_DEFAULTS)
+    return base_lm_architecture(args)
+
+
+ARCHS = {"transformer_lm": base_lm_architecture, "transformer_lm_t5": transformer_lm_t5}
+
+
+def _with_arch(args):
+    """A copy of `args` filled by its `arch` preset when that is transformer_lm_t5 (other arches: as given, missing
+    options taking base_lm_architecture's defaults where they are read)."""
+    if getattr(args, "arch", None) != "transformer_lm_t5":
+        return args
+    return transformer_lm_t5(Namespace(**vars(args)))
 
 
 def _opt(args, name, default):
@@ -72,7 +135,7 @@ class _Decoder(nn.Module):
         self.max_target_positions = args.max_target_positions
         if self.learned_pos:  # fairseq/modules/positional_embedding.py: max_positions + padding_idx + 1 rows
             self.embed_positions = nn.Embedding(args.max_target_positions + padding_idx + 1, C, padding_idx=padding_idx)
-        self.layers = nn.ModuleList([TransformerDecoderLayer(args, no_encoder_attn=True)
+        self.layers = nn.ModuleList([TransformerDecoderLayer(args, no_encoder_attn=True, head_dims=HEAD_DIMS)
                                      for _ in range(args.decoder_layers)])
         self.layer_norm = None if args.no_decoder_final_norm else nn.LayerNorm(C)
         self.output_projection = nn.Linear(C, vocab, bias=False)
@@ -87,13 +150,16 @@ class TransformerLM(nn.Module):
 
     def __init__(self, args, vocab_size, padding_idx=1):
         super().__init__()
+        args = _with_arch(args)
         bad = _unbuilt(args)
         if bad:
             raise NotImplementedError(f"transformer_lm options not built for LM fusion: {', '.join(bad)}")
         C = _opt(args, "decoder_embed_dim", 512)
         H = _opt(args, "decoder_attention_heads", 8)
-        if C != 64 * H:
-            raise NotImplementedError(f"LM heads of {C // H} dimensions: the attention kernels take 64")
+        if C % H != 0 or C // H not in HEAD_DIMS:
+            raise NotImplementedError(f"LM heads of {C / H:g} dimensions: the attention kernels take 64 and 80")
+        if C > MAX_DIM:
+            raise NotImplementedError(f"LM width {C}: the LayerNorm kernels take at most {MAX_DIM} channels")
         act = _opt(args, "activation_fn", "relu")
         if act not in ("relu", "gelu"):
             raise NotImplementedError(f"LM activation {act!r}: relu and gelu are built")

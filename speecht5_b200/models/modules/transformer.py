@@ -49,7 +49,7 @@ class MultiheadAttention(nn.Module):
     ops.linear (fused q|k|v projection) + ops.attention."""
 
     def __init__(self, embed_dim, num_heads, kdim=None, vdim=None, dropout=0.0, bias=True, self_attention=False,
-                 encoder_decoder_attention=False, has_relative_attention_bias=False):
+                 encoder_decoder_attention=False, has_relative_attention_bias=False, head_dims=(64,)):
         super().__init__()
         self.embed_dim = embed_dim
         self.kdim = kdim if kdim is not None else embed_dim
@@ -58,7 +58,9 @@ class MultiheadAttention(nn.Module):
         self.dropout_p = dropout
         self.head_dim = embed_dim // num_heads
         assert self.head_dim * num_heads == embed_dim, "embed_dim must be divisible by num_heads"
-        assert self.head_dim == 64, "the attention kernels are specialised for head_dim 64 (Base and Large)"
+        # head_dims: the widths this module may be built with. The speech model's attention (fused kernels, training) takes
+        # 64; the fusion LM (lm.TransformerLM, evaluation only) also 80, on the one-row kernel (ops.attention_rows).
+        assert self.head_dim in head_dims, f"head_dim {self.head_dim}: the attention kernels here take {head_dims}"
         self.scaling = self.head_dim ** -0.5
         self.self_attention = self_attention
         self.encoder_decoder_attention = encoder_decoder_attention
@@ -295,7 +297,7 @@ class TransformerEncoder(nn.Module):
 
 
 class TransformerDecoderLayer(nn.Module):
-    def __init__(self, args, no_encoder_attn=False, has_relative_attention_bias=False):
+    def __init__(self, args, no_encoder_attn=False, has_relative_attention_bias=False, head_dims=(64,)):
         super().__init__()
         self.embed_dim = args.decoder_embed_dim
         self.num_updates = 0
@@ -304,7 +306,7 @@ class TransformerDecoderLayer(nn.Module):
         # decoder self-attention has NO relative bias in the reference (transformer_layer.py:229-242, kwarg commented
         # out at :241): the position table and norm_k below are dead parameters kept for checkpoint compatibility.
         self.self_attn = MultiheadAttention(self.embed_dim, args.decoder_attention_heads,
-                                            dropout=args.attention_dropout, self_attention=True)
+                                            dropout=args.attention_dropout, self_attention=True, head_dims=head_dims)
         act = getattr(args, "activation_fn", None) or "relu"
         assert act in ("gelu", "relu")
         self.activation_fn = act

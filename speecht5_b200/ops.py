@@ -655,11 +655,25 @@ class ResidualLayerNormFn(torch.autograd.Function):
         return (dx if dx is not None else ds), (ds if has_res else None), dgamma, dbeta, None, None, None, None, None
 
 
+def _layer_norm_wide(x, residual, ln):
+    """LayerNorm(x + residual) over rows of 1024 < C <= 2048 channels on st5_ln_fwd_wide: evaluation only."""
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, residual, ln.weight, ln.bias)):
+        raise NotImplementedError(f"LayerNorm over {x.shape[-1]} channels has no backward (training takes C <= 1024)")
+    x = x.contiguous()
+    y = torch.empty_like(x)
+    K.ln_fwd_wide(x, residual.contiguous() if residual is not None else None, ln.weight.detach(), ln.bias.detach(), y,
+                  eps=ln.eps)
+    return y
+
+
 def residual_layer_norm(x, residual, ln, drop_p=0.0, stream=False):
     """stream=True (post-LN blocks, throughput mode): keep an fp32 copy of the output next to the bf16 activations and
     feed it to the next block's residual add, so that the residual stream is never rounded to bf16 between layers. The
     copy rides along as a plain attribute of the returned tensor (no autograd node: gradients flow through the bf16
     tensor exactly as before)."""
+    if x.shape[-1] > 1024:  # (st5_ln_fwd takes C <= 1024; wider rows have a forward-only kernel)
+        assert drop_p == 0.0
+        return _layer_norm_wide(x, residual, ln)
     res_f32 = getattr(residual, "_st5_f32", None) if residual is not None else None
     y_f32 = None
     if stream and RT.fp32_stream and x.dtype == torch.bfloat16 and x.is_cuda:
@@ -1072,19 +1086,43 @@ def attention_decode(q_buf, kv_buf, *, H, d, q_col, k_col, v_col, scale, key_pad
     query row b, or kv_div > 1 makes query row b read kv_buf row b // kv_div."""
     kvb = q_buf if kv_buf is None else kv_buf
     B, Tk = q_buf.shape[0], kvb.shape[1]
-    assert q_buf.shape[1] == 1 and d == H * 64 and q_buf.dtype == kvb.dtype
+    hd = d // H  # (64: st5_attn_decode_fwd / st5_attn_lineage_fwd; 80: their st5_*_hd_fwd counterparts)
+    assert q_buf.shape[1] == 1 and d == H * hd and hd in (64, 80) and q_buf.dtype == kvb.dtype
+    wide = {} if hd == 64 else dict(head_dim=hd)
     if kv_rows is not None or kv_div != 1:
         assert not return_probs
         out = torch.empty((B, 1, d), dtype=q_buf.dtype, device=q_buf.device)
-        K.attn_lineage_fwd(q_buf.narrow(2, q_col * d, d), kvb.narrow(2, k_col * d, d), kvb.narrow(2, v_col * d, d), out,
-                           H=H, scale=scale, key_pad=_key_pad_u8(key_pad), kv_rows=kv_rows, kv_div=kv_div)
+        (K.attn_lineage_fwd if hd == 64 else K.attn_lineage_hd_fwd)(
+            q_buf.narrow(2, q_col * d, d), kvb.narrow(2, k_col * d, d), kvb.narrow(2, v_col * d, d), out,
+            H=H, scale=scale, key_pad=_key_pad_u8(key_pad), kv_rows=kv_rows, kv_div=kv_div, **wide)
         return out, None
     assert kvb.shape[0] == B
     out = torch.empty((B, 1, d), dtype=q_buf.dtype, device=q_buf.device)
     probs = torch.empty((B, H, 1, Tk), dtype=torch.float32, device=q_buf.device) if return_probs else None
-    K.attn_decode_fwd(q_buf.narrow(2, q_col * d, d), kvb.narrow(2, k_col * d, d), kvb.narrow(2, v_col * d, d), out,
-                      H=H, scale=scale, key_pad=_key_pad_u8(key_pad), probs=probs)
+    (K.attn_decode_fwd if hd == 64 else K.attn_decode_hd_fwd)(
+        q_buf.narrow(2, q_col * d, d), kvb.narrow(2, k_col * d, d), kvb.narrow(2, v_col * d, d), out,
+        H=H, scale=scale, key_pad=_key_pad_u8(key_pad), probs=probs, **wide)
     return out, probs
+
+
+def attention_rows(q_buf, kv_buf, *, H, d, q_col, k_col, v_col, scale, key_pad=None, causal=False):
+    """Forward-only attention for heads the fused kernels do not take (80 channels): every query row of q_buf [B, Tq, *]
+    becomes one row of the one-row kernel over its utterance's keys (kv_div = Tq), with the causal mask and key_pad folded
+    into one [B*Tq, Tk] key mask. Returns (out [B, Tq, d], None)."""
+    if torch.is_grad_enabled() and (q_buf.requires_grad or (kv_buf is not None and kv_buf.requires_grad)):
+        raise NotImplementedError(f"attention over heads of {d // H} channels is forward-only (the fused attention "
+                                  "kernels and their backward take 64)")
+    kvb = q_buf if kv_buf is None else kv_buf
+    B, Tq, Tk = q_buf.shape[0], q_buf.shape[1], kvb.shape[1]
+    mask = torch.zeros((B, Tq, Tk), dtype=torch.bool, device=q_buf.device)
+    if causal:
+        mask |= torch.ones((Tq, Tk), dtype=torch.bool, device=q_buf.device).triu(1)
+    if key_pad is not None:
+        mask |= key_pad.bool()[:, None, :]
+    q_rows = q_buf.contiguous().view(B * Tq, 1, q_buf.shape[2])
+    out, _ = attention_decode(q_rows, kvb, H=H, d=d, q_col=q_col, k_col=k_col, v_col=v_col, scale=scale,
+                              key_pad=mask.view(B * Tq, Tk), kv_div=Tq)
+    return out.view(B, Tq, d), None
 
 
 def attention(q_buf, kv_buf, *, H, d, q_col, k_col, v_col, scale, pe_k=None, maxpos=0, key_pad=None, causal=False,
@@ -1093,6 +1131,10 @@ def attention(q_buf, kv_buf, *, H, d, q_col, k_col, v_col, scale, pe_k=None, max
             and not torch.is_grad_enabled():
         return attention_decode(q_buf, kv_buf, H=H, d=d, q_col=q_col, k_col=k_col, v_col=v_col, scale=scale,
                                 key_pad=key_pad, return_probs=return_probs)
+    if d != H * 64:  # (80-channel heads: forward only, on the one-row kernel)
+        assert pe_k is None and drop_p == 0.0 and not return_probs
+        return attention_rows(q_buf, kv_buf, H=H, d=d, q_col=q_col, k_col=k_col, v_col=v_col, scale=scale,
+                              key_pad=key_pad, causal=causal)
     # RT.probs_grad_heads: the consumer of the returned probabilities differentiates only through the first n heads (the
     # guided-attention loss; set by the trainer from the criterion): the backward skips the zero gradient of the others
     cfg = dict(H=H, d=d, q_col=q_col, k_col=k_col, v_col=v_col, scale=scale, maxpos=maxpos, causal=causal,

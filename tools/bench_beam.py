@@ -4,7 +4,11 @@ beam-1 GreedyGraph on the same inputs. The number of steps is fixed with min_len
 step, where it is the only choice), so an untrained model's outputs do not change the timing. Encoder included.
 
 With --lm, the same beam rows again with LM shallow fusion (`lm=`, `lm_weight` 0.5): a random-weight fairseq
-transformer_lm of base size (6 layers x 512, 8 heads, FFN 2048, vocabulary V - 2) run inside every captured step.
+transformer_lm of base size (6 layers x 512, 8 heads, FFN 2048, vocabulary V - 2) run inside every captured step, or with
+--lm-arch transformer_lm_t5 SpeechT5's own LM (20 layers x 1280, 16 heads of 80, FFN 6144, GELU); with it, the LM's
+key/value cache per bucket, the peak memory a beam decode allocates above the resident models, and the 80-wide
+st5_attn_lineage_hd_fwd alone at its full-size shape (8 sentences x K beams, 16 heads, a lineage table over 256 cached
+positions) with bytes per second from shapes.
 
 Also CUDA-event times of st5_beam_topk (and, with --lm, st5_beam_topk_lm at V_lm = V - 2) and st5_beam_update alone (V = 81 and V = 8 000, the ASR character and the
 MuST-C ST vocabularies) and of st5_attn_lineage_fwd at the 10 s cross-attention shape (8 sentences x K beams over one
@@ -42,6 +46,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=64, help="decoder steps per decode (min_len = max_len)")
     ap.add_argument("--lm", action="store_true", help="also the LM-fusion rows")
+    ap.add_argument("--lm-arch", default="transformer_lm", choices=("transformer_lm", "transformer_lm_t5"),
+                    help="the LM of the --lm rows: base transformer_lm (6 x 512) or transformer_lm_t5 (20 x 1280)")
     args = ap.parse_args()
     import torch
     from speecht5_b200 import kernels
@@ -72,15 +78,27 @@ def main():
         from argparse import Namespace
         from speecht5_b200.lm import TransformerLM
         V = asr.text_decoder_postnet.output_projection.weight.shape[0]
-        lm = TransformerLM(Namespace(decoder_layers=6, decoder_embed_dim=512, decoder_attention_heads=8,
-                                     decoder_ffn_embed_dim=2048), V - 2)
+        if args.lm_arch == "transformer_lm_t5":
+            lm = TransformerLM(Namespace(arch="transformer_lm_t5"), V - 2)
+        else:
+            lm = TransformerLM(Namespace(decoder_layers=6, decoder_embed_dim=512, decoder_attention_heads=8,
+                                         decoder_ffn_embed_dim=2048), V - 2)
         for p in lm.parameters():
             torch.nn.init.normal_(p, std=0.05)
         lm = lm.to(dev)
+        out["lm_arch"] = args.lm_arch
         for K in (5, 10):
+            torch.cuda.synchronize()
+            resident = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
             ms8 = cuda_ms(lambda: asr.generate_text_beam(wav, wpm, beam_size=K, use_cache="graph", lm=lm, lm_weight=0.5,
                                                          **kw))
-            out[f"beam{K}_lm_graph"] = dict(ms_B8=ms8, ms_per_step_B8=ms8 / (n + 1), utt_per_s_B8=8 / (ms8 / 1e3))
+            row = dict(ms_B8=ms8, ms_per_step_B8=ms8 / (n + 1), utt_per_s_B8=8 / (ms8 / 1e3))
+            if args.lm_arch == "transformer_lm_t5":
+                bg = [g for key, g in asr.__dict__.get("_beam_graphs", {}).items() if key[1] == K and g.lm is lm]
+                row["lm_cache_MiB"] = sum(c.numel() * c.element_size() for c in bg[0].lm_cache.self_kv) / 2 ** 20
+                row["peak_above_resident_MiB"] = (torch.cuda.max_memory_allocated() - resident) / 2 ** 20
+            out[f"beam{K}_lm_graph"] = row
     del asr
     # kernels alone
     B, t = 8, torch.tensor([5], dtype=torch.int64, device=dev)
@@ -130,6 +148,22 @@ def main():
         # each query row reads its sentence's keys and values (L2 serves the K-fold reuse; this counts what is read)
         nbytes = B * K * S * 2 * H * 64 * 2 + q.numel() * 2 * 2 + pad.numel()
         out[f"attn_lineage_cross_K{K}"] = dict(us=us, GBps=nbytes / (us * 1e-6) / 1e9)
+    if args.lm and args.lm_arch == "transformer_lm_t5":
+        H, hd, T = 16, 80, 256  # (transformer_lm_t5's self-attention: 16 heads of 80, 256 cached positions)
+        for K in (5, 10):
+            BK, rows = B * K, T + 9
+            q = torch.randn(BK, 1, 3 * H * hd, device=dev).to(torch.bfloat16)
+            cache = torch.randn(BK, rows, 2 * H * hd, device=dev).to(torch.bfloat16)
+            o = torch.empty(BK, 1, H * hd, device=dev, dtype=torch.bfloat16)
+            pad = torch.zeros(BK, T, dtype=torch.uint8, device=dev)
+            # a lineage table as beam reorders leave it: each position from some beam row of the same sentence
+            lin = (torch.arange(BK, device=dev)[:, None] // K * K
+                   + torch.randint(0, K, (BK, rows), device=dev)).to(torch.int32)
+            us = 1e3 * cuda_ms(lambda: kernels.attn_lineage_hd_fwd(
+                q[:, :, :H * hd], cache[:, :T, :H * hd], cache[:, :T, H * hd:], o, H=H, head_dim=hd, scale=hd ** -0.5,
+                key_pad=pad, kv_rows=lin), reps=200)
+            nbytes = BK * T * 2 * H * hd * 2 + BK * H * hd * 2 * 2 + pad.numel() + BK * T * 4
+            out[f"attn_lineage_hd80_self_K{K}_T{T}"] = dict(us=us, GBps=nbytes / (us * 1e-6) / 1e9)
     print(json.dumps(out))
 
 
