@@ -60,23 +60,26 @@ def _act_grad(z, act):
     raise AssertionError(act)
 
 
-def gemm_keep(M, N, nb, drop_p, seed, offset):
+def gemm_keep(M, N, nb, drop_p, seed, offset, rows=None, cols=None):
     """[nb, M, N] keep mask of the GEMM epilogue's dropout: element (z, m, n) has index (z * M + m) * N + n -- the logical
-    output, whatever c_ld and the batch strides are (tests/dropout_ref.py states the generator)."""
+    output, whatever c_ld and the batch strides are (tests/dropout_ref.py states the generator). rows / cols (index
+    tensors): the [nb, len(rows), len(cols)] part of it only."""
     import numpy as np
     import dropout_ref
-    idx = (np.arange(nb, dtype=np.uint64)[:, None, None] * np.uint64(M) + np.arange(M, dtype=np.uint64)[:, None]) \
-        * np.uint64(N) + np.arange(N, dtype=np.uint64)
+    r = np.arange(M, dtype=np.uint64) if rows is None else rows.numpy().astype(np.uint64)
+    c = np.arange(N, dtype=np.uint64) if cols is None else cols.numpy().astype(np.uint64)
+    idx = (np.arange(nb, dtype=np.uint64)[:, None, None] * np.uint64(M) + r[:, None]) * np.uint64(N) + c
     return torch.from_numpy(dropout_ref.keep_mask(seed, offset, idx, drop_p))
 
 
 def gemm(a, b, out, *, M, N, K, a_mn=False, b_mn=False, a_ld=None, b_ld=None, c_ld=None, nb1=1, nb2=1, a_bs=(0, 0),
          b_bs=(0, 0), c_bs=(0, 0), bias=None, bias2=None, bias2_rows=0, residual=None, c_pre=None, act=None, alpha=1.0,
-         accumulate=False, drop_p=0.0, seed=0, offset=0, actgrad_pre=None, actgrad_act=None):
+         accumulate=False, drop_p=0.0, seed=0, offset=0, actgrad_pre=None, actgrad_act=None, rows=None, cols=None):
     """st5_gemm_bf16 in fp64: out[z] = dropout(act(alpha * A[z] B[z]^T + c_old + bias + bias2)) * act'(actgrad_pre)
     + residual, z = b2 * nb1 + b1; c_pre receives the value before act() (for gelu_tanh_gate: keep * scale *
     gelu_tanh'(x) instead). bias2 row m is bias2[m // bias2_rows] at a row pitch of N, the same for every batch entry
-    (the kernel does not index it by z)."""
+    (the kernel does not index it by z). rows / cols (index tensors into [M) / [N)): compute and write only the outputs
+    (z, rows[i], cols[j]) -- every output depends on its own row of A and column of B^T only, over the full K."""
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
     assert not (int(offset) >> 63), "device-resident seeds: pass the seed value itself"
     a_ld = a_ld if a_ld is not None else (M if a_mn else K)
@@ -86,12 +89,22 @@ def gemm(a, b, out, *, M, N, K, a_mn=False, b_mn=False, a_ld=None, b_ld=None, c_
         assert (t.storage_offset() * 2) % 16 == 0 and (ld * 2) % 16 == 0, "TMA alignment"
         assert (bs[0] * 2) % 16 == 0 and (bs[1] * 2) % 16 == 0, "TMA alignment"
     nb = nb1 * nb2
-    A = _view(a, nb1, M, K, a_mn, a_ld, a_bs[0], nb2, a_bs[1]).double()
-    B = _view(b, nb1, N, K, b_mn, b_ld, b_bs[0], nb2, b_bs[1]).double()
-    v = (alpha * torch.bmm(A, B.transpose(1, 2))).reshape(nb2, nb1, M, N)
+    rr = torch.arange(M) if rows is None else rows
+    cc = torch.arange(N) if cols is None else cols
+    A = _view(a, nb1, M, K, a_mn, a_ld, a_bs[0], nb2, a_bs[1])[:, rr].double()
+    B = _view(b, nb1, N, K, b_mn, b_ld, b_bs[0], nb2, b_bs[1])[:, cc].double()
+    Mr, Nc = len(rr), len(cc)
+    v = (alpha * torch.bmm(A, B.transpose(1, 2))).reshape(nb2, nb1, Mr, Nc)
+    sub = (slice(None), slice(None), rr[:, None], cc[None, :])
 
     def out_view(t):
         return torch.as_strided(t, (nb2, nb1, M, N), (c_bs[1], c_bs[0], c_ld, 1), t.storage_offset())
+
+    def read(t):
+        return out_view(t)[sub]
+
+    def write(t, val):
+        out_view(t)[sub] = val.to(t.dtype)
     shared = (nb1 > 1 and c_bs[0] == 0) or (nb2 > 1 and c_bs[1] == 0)
     if int(accumulate) == 2:  # L2-side accumulate: batch entries may share one output (c_bs = 0), split-K
         assert out.dtype == torch.float32 and (c_ld * 4) % 16 == 0 and bias is None and c_pre is None and act in (None, "none")
@@ -99,38 +112,37 @@ def gemm(a, b, out, *, M, N, K, a_mn=False, b_mn=False, a_ld=None, b_ld=None, c_
         C = out_view(out)
         for b2 in range(nb2):
             for b1 in range(nb1):
-                C[b2, b1].copy_((C[b2, b1].double() + v[b2, b1]).to(out.dtype))
+                C[b2, b1][sub[2:]] = (C[b2, b1][sub[2:]].double() + v[b2, b1]).to(out.dtype)
         return out
     assert not shared, "several batch entries into one output need accumulate = 2"
     assert not (accumulate and out.dtype == torch.bfloat16), "accumulate needs an fp32 output"
-    C = out_view(out)
     if accumulate:
-        v = v + C.double()
+        v = v + read(out).double()
     if bias is not None:
         assert bias.dtype == torch.float32
-        v = v + bias[:N].double()
+        v = v + bias[:N][cc].double()
     if bias2 is not None:  # per-utterance bias: row m takes bias2[m // bias2_rows], row pitch N
         assert bias2.dtype == torch.float32 and bias2_rows > 0
         flat = bias2.reshape(-1).double()
-        v = v + flat[(torch.arange(M) // bias2_rows)[:, None] * N + torch.arange(N)]
-    keep = gemm_keep(M, N, nb, drop_p, seed, offset).reshape(nb2, nb1, M, N) if drop_p > 0 else None
+        v = v + flat[(rr // bias2_rows)[:, None] * N + cc]
+    keep = gemm_keep(M, N, nb, drop_p, seed, offset, rows, cols).reshape(nb2, nb1, Mr, Nc) if drop_p > 0 else None
     scale = 1.0 / (1.0 - drop_p) if drop_p > 0 else 1.0
     if act == "gelu_tanh_gate":
         assert c_pre is not None and out.dtype == torch.bfloat16 and N % 8 == 0
         second = _gelu_tanh_grad(v) * (keep * scale if keep is not None else 1.0)  # the backward multiplier
-        out_view(c_pre).copy_(second.to(c_pre.dtype))
+        write(c_pre, second)
     elif c_pre is not None:
-        out_view(c_pre).copy_(v.to(c_pre.dtype))
+        write(c_pre, v)
     v = _act(v, act)
     if keep is not None:
         v = torch.where(keep, v * scale, torch.zeros_like(v))
     if actgrad_pre is not None:  # activation backward fused into the product: v *= act'(pre[m][n])
-        pre = out_view(actgrad_pre).double()
+        pre = read(actgrad_pre).double()
         v = v * (pre if actgrad_act == "gate" else _act_grad(pre, actgrad_act))
     if residual is not None:  # same layout and dtype as C, added after the activation
         assert residual.dtype == out.dtype
-        v = v + out_view(residual).double()
-    C.copy_(v.to(out.dtype))
+        v = v + read(residual).double()
+    write(out, v)
     return out
 
 

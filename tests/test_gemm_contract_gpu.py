@@ -40,7 +40,11 @@ class Operand:
     the padding columns / rows up to ld and the gaps between padded batch entries are NaN, so reading them poisons the
     product."""
 
-    def __init__(self, rows, K, mn, nb1=1, nb2=1, bcast1=False, bcast2=False, gen=None, scale=1.0, dev="cuda"):
+    def __init__(self, rows, K, mn, nb1=1, nb2=1, bcast1=False, bcast2=False, gen=None, scale=1.0, dev="cuda",
+                 lay=None):
+        if lay is not None:
+            self._recorded(rows, K, mn, nb1, nb2, lay, gen, scale, dev)
+            return
         ext = rows if mn else K
         self.ld = _r8(ext) + 8
         inner = (K if mn else rows) * self.ld
@@ -57,6 +61,22 @@ class Operand:
         self.cpu = buf.to(torch.bfloat16)
         self.dev = self.cpu.to(dev)
         self.mn = mn
+
+    def _recorded(self, rows, K, mn, nb1, nb2, lay, gen, scale, dev):
+        """lay = (ld, bs1, bs2, off): a layout taken from a real launch (overlapping batch entries, interleaved heads or
+        windows included). Every element the operand covers is random, everything else NaN; the operand starts `off`
+        elements past a 128-byte boundary, after a NaN guard zone."""
+        self.ld, self.bs1, self.bs2, off = lay
+        self.mn = mn
+        outer, inner = (K, rows) if mn else (rows, K)
+        o = 64 + off
+        idx = (o + torch.arange(nb2)[:, None, None, None] * self.bs2 + torch.arange(nb1)[None, :, None, None] * self.bs1
+               + torch.arange(outer)[:, None] * self.ld + torch.arange(inner)).reshape(-1)
+        buf = torch.full((int(idx.max()) + 65,), NAN, dtype=torch.float32)
+        buf[idx] = torch.randn(idx.numel(), generator=gen) * scale
+        buf = buf.to(torch.bfloat16)
+        self.cpu = buf[o:]
+        self.dev = buf.to(dev)[o:]
 
     def kw(self, which):
         return {f"{which}_mn": self.mn, f"{which}_ld": self.ld, f"{which}_bs": (self.bs1, self.bs2)}
@@ -86,17 +106,21 @@ class OutLayout:
     """Logical [nb2][nb1][M][N] region at pitch c_ld inside a larger buffer (rows past M, columns past N, gaps between
     batch entries and guard zones before and after); `inside` marks the logical elements."""
 
-    def __init__(self, M, N, nb1=1, nb2=1, c_ld=None, shared=False, misalign=0):
+    def __init__(self, M, N, nb1=1, nb2=1, c_ld=None, shared=False, misalign=0, bs=None):
+        """bs: batch strides taken from a real launch (interleaved heads or a shared output included)."""
         self.M, self.N, self.nb1, self.nb2 = M, N, nb1, nb2
         self.c_ld = c_ld if c_ld is not None else _r8(N) + 8
         self.bs1 = 0 if (shared or nb1 == 1) else (M + 3) * self.c_ld
         self.bs2 = 0 if (shared or nb2 == 1) else (self.bs1 * nb1 if self.bs1 else (M + 3) * self.c_ld) + 8 * self.c_ld
+        if bs is not None:
+            self.bs1, self.bs2 = bs
         self.base = 32 + misalign
-        self.size = self.base + (nb2 - 1) * self.bs2 + (nb1 - 1) * self.bs1 + (M + 3) * self.c_ld + 64
         b2 = torch.arange(nb2)[:, None, None, None] * self.bs2
         b1 = torch.arange(nb1)[None, :, None, None] * self.bs1
         idx = self.base + b2 + b1 + torch.arange(M)[:, None] * self.c_ld + torch.arange(N)
         self.idx = idx  # [nb2, nb1, M, N] flat positions
+        self.size = max(self.base + (nb2 - 1) * self.bs2 + (nb1 - 1) * self.bs1 + (M + 3) * self.c_ld,
+                        int(idx.max()) + 1) + 64
         self.inside = torch.zeros(self.size, dtype=torch.bool)
         self.inside[idx.reshape(-1)] = True
 
@@ -128,30 +152,45 @@ def _act_f64(v, act):
 def run_gemm(M, N, K, *, a_mn=False, b_mn=False, nb1=1, nb2=1, a_bcast=(False, False), b_bcast=(False, False),
              out_dtype=torch.float32, c_ld=None, shared=False, misalign=0, alpha=1.0, accumulate=0, bias=None,
              bias2_rows=0, residual=False, c_pre=False, act=None, actgrad_act=None, drop_p=0.0, seed=1234,
-             offset=7, device_seed=False, operand_scale=None, seed_data=0, check=True, a_win=None, b_win=None):
+             offset=7, device_seed=False, operand_scale=None, seed_data=0, check=True, a_win=None, b_win=None,
+             a_lay=None, b_lay=None, c_bs=None, residual_is_out=False, blocks=None, bias2_off=0, dev="cuda"):
     """Run K.gemm on NaN-guarded buffers, then compare with the fp64 statement elementwise. Returns a dict of the CPU
     results (got / ref regions, pre-activation, keep mask) for case-specific checks. a_win / b_win: the row pitch of
-    an overlapping-window operand (WindowOperand, nb2 = 1)."""
+    an overlapping-window operand (WindowOperand, nb2 = 1).
+
+    A launch recorded from a real update is replayed with its own layout: a_lay / b_lay = (ld, bs1, bs2, element
+    offset from a 16-byte boundary), c_ld / c_bs / misalign for the output (c_pre, residual and actgrad_pre share its
+    layout), residual_is_out for an in-place residual (residual = out), bias and bias2_off element offsets. blocks: a list of (rows, cols) index tensors (None: all) -- the fp64
+    statement is evaluated and compared on those outputs only (every batch entry, full K); the sentinels are checked
+    everywhere."""
     from speecht5_b200 import kernels as K_
-    dev = torch.device("cuda")
+    dev = torch.device(dev)
     gen = torch.Generator().manual_seed(seed_data)
     # operand scale: the pre-activation has unit standard deviation whatever K is
     sc = operand_scale if operand_scale is not None else K ** -0.25
-    A = WindowOperand(M, K, a_mn, a_win, nb1, gen=gen, scale=sc) if a_win else \
-        Operand(M, K, a_mn, nb1, nb2, *a_bcast, gen=gen, scale=sc)
-    B = WindowOperand(N, K, b_mn, b_win, nb1, gen=gen, scale=sc) if b_win else \
-        Operand(N, K, b_mn, nb1, nb2, *b_bcast, gen=gen, scale=sc)
-    L = OutLayout(M, N, nb1, nb2, c_ld=c_ld, shared=shared, misalign=misalign)
-    c0 = L.buffer(out_dtype, fill="randn" if accumulate == 1 else ("zero" if accumulate == 2 else None), gen=gen)
+    A = WindowOperand(M, K, a_mn, a_win, nb1, gen=gen, scale=sc, dev=dev) if a_win else \
+        Operand(M, K, a_mn, nb1, nb2, *a_bcast, gen=gen, scale=sc, dev=dev, lay=a_lay)
+    B = WindowOperand(N, K, b_mn, b_win, nb1, gen=gen, scale=sc, dev=dev) if b_win else \
+        Operand(N, K, b_mn, nb1, nb2, *b_bcast, gen=gen, scale=sc, dev=dev, lay=b_lay)
+    L = OutLayout(M, N, nb1, nb2, c_ld=c_ld, shared=shared, misalign=misalign, bs=c_bs)
+    c0 = L.buffer(out_dtype, fill="randn" if (accumulate == 1 or residual_is_out) else
+                  ("zero" if accumulate == 2 else None), gen=gen)
     if accumulate == 2 and shared:
         c0[L.idx[0, 0].reshape(-1)] = torch.randn(M * N, generator=gen).to(out_dtype)
-    bias_t = bias2_t = None
+    elif accumulate == 2 and c_bs is not None:  # a recorded reduce-add: the output starts non-zero
+        c0[L.idx.reshape(-1)] = torch.randn(L.idx.numel(), generator=gen).to(out_dtype)
+    # bias / bias2: CPU views for the fp64 statement, and device views at the same element offset into a buffer that
+    # is copied whole (a copy of the view alone would start 16-byte aligned again)
+    bias_t = bias2_t = bias_d = bias2_d = None
     if bias is not None:
         bb = torch.randn(N + 8, generator=gen)
-        bias_t = bb[1:N + 1] if bias == "offset" else bb[:N]  # "offset": 4 bytes past a 16-byte boundary
+        o = 1 if bias == "offset" else (0 if bias == "aligned" else bias)  # "offset": 4 bytes past a 16-byte boundary
+        bias_t, bias_d = bb[o:N + o], bb.to(dev)[o:N + o]
     if bias2_rows:
-        bias2_t = torch.randn((M + bias2_rows - 1) // bias2_rows, N, generator=gen)
-    res_t = L.buffer(out_dtype, fill="randn", gen=gen) if residual else None
+        n2 = (M + bias2_rows - 1) // bias2_rows
+        b2 = torch.randn(n2 * N + 8, generator=gen)
+        bias2_t, bias2_d = (t[bias2_off:bias2_off + n2 * N].view(n2, N) for t in (b2, b2.to(dev)))
+    res_t = c0 if residual_is_out else (L.buffer(out_dtype, fill="randn", gen=gen) if residual else None)
     ag_t = None
     if actgrad_act is not None:
         ag_t = L.buffer(out_dtype, fill="randn", gen=gen, scale=0.7)
@@ -163,50 +202,75 @@ def run_gemm(M, N, K, *, a_mn=False, b_mn=False, nb1=1, nb2=1, a_bcast=(False, F
     def dv(t):
         return None if t is None else t.to(dev)
     # ---- device run
-    cd = c0.to(dev)
+    cd = c0.to(dev, copy=True)  # (a copy on the CPU too: c0 is the reference's starting point)
     out_d = cd[L.base:]
+    if residual_is_out:
+        res_d = cd
     kseed, koff = seed, offset
     if device_seed:
         seed_buf = torch.tensor([seed], dtype=torch.int64, device=dev)
         kseed, koff = seed_buf.data_ptr(), offset | (1 << 63)
     pre_d = dv(pre_t)
-    res_d, ag_d = dv(res_t), dv(ag_t)
-    K_.gemm(A.dev, B.dev, out_d, **common, bias=dv(bias_t), bias2=dv(bias2_t), bias2_rows=bias2_rows,
+    if not residual_is_out:
+        res_d = dv(res_t)
+    ag_d = dv(ag_t)
+    K_.gemm(A.dev, B.dev, out_d, **common, bias=bias_d, bias2=bias2_d, bias2_rows=bias2_rows,
             residual=None if res_d is None else res_d[L.base:], c_pre=None if pre_d is None else pre_d[L.base:],
             actgrad_pre=None if ag_d is None else ag_d[L.base:], actgrad_act=actgrad_act, seed=kseed, offset=koff)
-    torch.cuda.synchronize()
+    if dev.type == "cuda":
+        torch.cuda.synchronize()
     got = cd.cpu()
     got_pre = pre_d.cpu() if pre_d is not None else None
     # ---- fp64 statement
     ref = c0.clone()
     ref_pre = L.buffer(out_dtype) if c_pre else None
-    E.gemm(A.cpu, B.cpu, ref[L.base:], **common, bias=bias_t, bias2=bias2_t, bias2_rows=bias2_rows,
-           residual=None if res_t is None else res_t[L.base:], c_pre=None if ref_pre is None else ref_pre[L.base:],
-           actgrad_pre=None if ag_t is None else ag_t[L.base:], actgrad_act=actgrad_act, seed=seed, offset=offset)
     # exact pre-activation v + c_old + bias + bias2, and |alpha| |A| |B|^T, in fp64
     pre64 = c0.double() if accumulate == 1 else L.buffer(torch.float64, fill="zero")
     plain = dict(common, act=None, drop_p=0.0, accumulate=1 if accumulate == 1 else 0)
-    if accumulate != 2:
-        E.gemm(A.cpu, B.cpu, pre64[L.base:], **plain, bias=bias_t, bias2=bias2_t, bias2_rows=bias2_rows)
     mag = L.buffer(torch.float32, fill="zero")
     magkw = dict(plain, alpha=abs(alpha), accumulate=2 if accumulate == 2 else 0)
-    E.gemm(A.cpu.float().abs().to(torch.bfloat16), B.cpu.float().abs().to(torch.bfloat16), mag[L.base:], **magkw)
-    r = dict(L=L, got=L.region(got).double(), ref=L.region(ref).double(), pre=L.region(pre64).double(),
-             mag=L.region(mag).double(), got_buf=got, ref_buf=ref, got_pre=got_pre, ref_pre=ref_pre)
+    a_abs, b_abs = A.cpu.float().abs().to(torch.bfloat16), B.cpu.float().abs().to(torch.bfloat16)
+    sel, parts = None, [(None, None)]  # the outputs compared (all, or the union of the blocks), as disjoint parts
+    if blocks:
+        sel = torch.zeros(nb2, nb1, M, N, dtype=torch.bool)
+        for rows, cols in blocks:
+            sel[:, :, slice(None) if rows is None else rows[:, None], slice(None) if cols is None else cols] = True
+        pattern, which = torch.unique(sel[0, 0], dim=0, return_inverse=True)  # rows with the same columns: one part
+        parts = [((which == i).nonzero()[:, 0], p.nonzero()[:, 0]) for i, p in enumerate(pattern) if p.any()]
+    for rows, cols in parts:  # (disjoint: accumulating statements must see every output once)
+        E.gemm(A.cpu, B.cpu, ref[L.base:], **common, bias=bias_t, bias2=bias2_t, bias2_rows=bias2_rows,
+               residual=None if res_t is None else res_t[L.base:], c_pre=None if ref_pre is None else ref_pre[L.base:],
+               actgrad_pre=None if ag_t is None else ag_t[L.base:], actgrad_act=actgrad_act, seed=seed, offset=offset,
+               rows=rows, cols=cols)
+        if accumulate != 2:
+            E.gemm(A.cpu, B.cpu, pre64[L.base:], **plain, bias=bias_t, bias2=bias2_t, bias2_rows=bias2_rows,
+                   rows=rows, cols=cols)
+        E.gemm(a_abs, b_abs, mag[L.base:], **magkw, rows=rows, cols=cols)
+
+    def region(buf):
+        x = L.region(buf)
+        return x if sel is None else x[sel]
+    r = dict(L=L, got=region(got).double(), ref=region(ref).double(), pre=region(pre64).double(),
+             mag=region(mag).double(), got_buf=got, ref_buf=ref, got_pre=got_pre, ref_pre=ref_pre, sel=sel)
     if drop_p > 0:
-        r["keep"] = E.gemm_keep(M, N, nb1 * nb2, drop_p, seed, offset).reshape(nb2, nb1, M, N)
+        if sel is None:
+            r["keep"] = E.gemm_keep(M, N, nb1 * nb2, drop_p, seed, offset).reshape(nb2, nb1, M, N)
+        else:
+            import numpy as np
+            z, m, n = (t.numpy().astype(np.uint64) for t in (sel.reshape(-1, M, N).nonzero().T))
+            r["keep"] = torch.from_numpy(D.keep_mask(seed, offset, (z * np.uint64(M) + m) * np.uint64(N) + n, drop_p))
     if not check:
         return r
     # ---- bound
     scale = D.drop_scale(drop_p) if drop_p > 0 else 1.0
     agmax = 1.0
     if ag_t is not None:
-        agp = L.region(ag_t).double()
+        agp = region(ag_t).double()
         agmax = float(agp.abs().max()) if actgrad_act == "gate" else 1.2
     amp = 1.2 * scale * agmax
     addmag = r["pre"].abs()
     if accumulate in (1, 2):
-        addmag = addmag + L.region(c0).double().abs()
+        addmag = addmag + region(c0).double().abs()
     bound = C_ACC * 2.0 ** -24 * math.sqrt(K) * r["mag"] * amp + 2.0 ** -20 * addmag * amp + TINY
     if act in ("gelu_tanh", "gelu_tanh_gate"):  # MUFU tanh.approx: |error| <= 2^-11 |tanh|
         bound = bound + 2.0 ** -10 * (1 + r["pre"].abs()) * scale * agmax
@@ -214,22 +278,28 @@ def run_gemm(M, N, K, *, a_mn=False, b_mn=False, nb1=1, nb2=1, a_bcast=(False, F
         v = _act_f64(r["pre"], act).abs() * scale
         bound = bound + 2.0 ** -8 * v
     if res_t is not None:
-        bound = bound + 2.0 ** -22 * L.region(res_t).double().abs()
+        bound = bound + 2.0 ** -22 * region(res_t).double().abs()
     if out_dtype == torch.bfloat16:  # got and ref are both rounded to bf16: one unit in the last place apart at most
         bound = bound + 2.0 ** -7 * r["ref"].abs()
     err = (r["got"] - r["ref"]).abs()
     bad = ~(err <= bound)
-    assert not bool(bad.any()), (f"{int(bad.sum())} of {bad.numel()} outputs off; first (b2, b1, m, n) = "
-                                 f"{tuple(int(i) for i in bad.nonzero()[0])}, max err/bound "
-                                 f"{float((err / bound)[~torch.isnan(err)].max()):.3g}")
+    r["worst"] = float((err / bound).nan_to_num(math.inf).max()) if err.numel() else 0.0
+    if bool(bad.any()):
+        first = bad.nonzero()[0] if sel is None else sel.nonzero()[int(bad.nonzero()[0])]
+        raise AssertionError(f"{int(bad.sum())} of {bad.numel()} outputs off; first (b2, b1, m, n) = "
+                             f"{tuple(int(i) for i in first)}, max err/bound {r['worst']:.3g}")
     L.assert_outside_untouched(got)
+    if sel is not None:  # outputs outside the compared blocks: written at least
+        unwritten = ~torch.isfinite(L.region(got).float())
+        assert not bool(unwritten.any()), f"output (b2, b1, m, n) = {tuple(int(i) for i in unwritten.nonzero()[0])} " \
+                                          "not written"
     if c_pre:
         L.assert_outside_untouched(got_pre, "c_pre")
         if act != "gelu_tanh_gate":  # the pre-activation itself
             pb = C_ACC * 2.0 ** -24 * math.sqrt(K) * r["mag"] * 1.2 + 2.0 ** -20 * addmag + TINY
             if out_dtype == torch.bfloat16:
                 pb = pb + 2.0 ** -8 * r["pre"].abs()
-            e = (L.region(got_pre).double() - r["pre"]).abs()
+            e = (region(got_pre).double() - r["pre"]).abs()
             assert bool((e <= pb).all()), f"c_pre off at {tuple(int(i) for i in (e > pb).nonzero()[0])}"
     if drop_p > 0:
         before = _act_f64(r["pre"], act)
